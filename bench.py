@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py — PDLP iterations/sec on BASELINE.json's headline workload: the synthetic sparse LP with 10M variables x
-10M constraints, 8 nnz/row, fp64 (configs[3]'s instance; it fits one B200, so every N = 1, 2, 4, 8 runs the SAME LP and
-the N-GPU numbers are strong scaling).  --workload c2 selects configs[1] (1M x 1M), --workload c3 the pds-shaped
+10M constraints, 8 nnz/row, fp64 (configs[3]'s instance; it fits one 80 GB H100, so every N = 1, 2, 4, 8 runs the SAME LP
+and the N-GPU numbers are strong scaling).  --workload c2 selects configs[1] (1M x 1M), --workload c3 the pds-shaped
 multicommodity LP of configs[2] (both single-GPU profile workloads).
 
   python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path (through the C ABI)
@@ -11,7 +11,9 @@ A "step" = one solve of ITERS_PER_STEP PDLP iterations on the resident LP (toler
   value  = accepted PDLP iterations / device time of the solver loop (CUDA events, inputs resident in HBM)
   e2e    = the same through cuOptCreateRangedProblem + cuOptSolve + cuOptGet*Solution with HOST buffers:
            H2D upload, transpose, diagonal scaling and D2H of the solution are inside the timed region
-Prints ONE JSON line (rank 0).
+Prints ONE JSON line (rank 0).  --dump-outputs DIR also writes what the last timed step returned to the caller (primal,
+dual, reduced costs: a fixed, seeded sample of 2^21 entries each when longer; objectives and iterations) as
+DIR/<name>.npy; with several GPUs, rank 0 writes its own (its rows of the dual).
 """
 from __future__ import annotations
 
@@ -66,11 +68,11 @@ def measured_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return json.load(f), "measured"
     except Exception:  # noqa: BLE001
-        return {"hbm_gbs": 6650.0}, "fallback"
+        return {"hbm_gbs": 3350.0}, "H100 SXM data sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -106,16 +108,7 @@ class ClockSampler:
 
 
 WORKLOADS = {"c4": (10_000_000, 10_000_000), "c2": (1_000_000, 1_000_000)}
-# dram__bytes_read.sum + dram__bytes_write.sum per step of the dominant kernel (group), from the COMMITTED `ncu --set full`
-# captures under profiles/ (bench.py never runs under a profiler): (workload, kernel, blocked) -> (bytes, file).  The line
-# says `traffic_source: committed capture` so that nobody mistakes it for an in-run measurement.
-NCU_TRAFFIC = {}
-try:
-    with open(os.path.join(ROOT, "profiles", "r2", "ncu_traffic.json")) as _f:
-        for _e in json.load(_f)["entries"]:
-            NCU_TRAFFIC[(_e["workload"], _e["kernel"], bool(_e["blocked"]))] = (_e["bytes_per_step"], _e["source"])
-except Exception:  # noqa: BLE001
-    pass
+DUMP_SAMPLE = 1 << 21  # entries kept per dumped vector: 3 vectors x 2^21 doubles = 48 MB
 TRANSPORTS = {"gather": "every rank owns 1/N of the rows of A and 1/N of the rows of A^T; xbar and y' are all-gathered by NVLink "
                         "peer stores issued by the kernels that produce them (K1, K2), 3 scalars per rank; no partial "
                         "products, no NCCL inside the PDHG loop",
@@ -135,7 +128,7 @@ def workload(args):
     return lpgen.sparse_lp(args.rows or rows, args.cols or cols, args.nnz_per_row, seed=1234, locality=args.locality)
 
 
-def config_dict(args, lp, n_gpus):
+def config_dict(args, lp, n_gpus, l2_bytes=None):
     names = {"c4": "configs[3] instance (the 10M-var LP the metric is quoted on)", "c2": "configs[1]",
              "c3": "configs[2] (pds-shaped multicommodity flow, synthesised: no pds file in the tree)"}
     transport = os.environ.get("CUOPT_B200_DIST_MODE", "gather")
@@ -144,8 +137,9 @@ def config_dict(args, lp, n_gpus):
             "pdlp_solver_mode": "Stable2",
             "parallelism": (f"ONE LP: constraint rows and primal column slices sharded over {n_gpus} GPUs (one process "
                             f"each); transport: {TRANSPORTS[transport]}") if n_gpus > 1 else "1 GPU",
-            "l2_policy": "per-iteration working set (A, A^T, 14 vectors = %.0f MB) exceeds the 126 MB L2"
-                         % (lp.algorithmic_bytes_per_iteration() / 1e6)}
+            "l2_policy": "per-iteration working set (A, A^T, 14 vectors = %.0f MB) against the %s L2"
+                         % (lp.algorithmic_bytes_per_iteration() / 1e6,
+                            "%.0f MB" % (l2_bytes / 1e6) if l2_bytes else "device's")}
 
 
 def time_cpu_oracle(lp, cores, iterations, repeats):
@@ -222,6 +216,25 @@ def cusparse_comparator(lp, timeout_s=240):
     return None
 
 
+def dump_outputs(out_dir, x, y, rc, st):
+    """What the caller of the timed path received in the last timed step, as float64 .npy files.  Vectors longer than
+    DUMP_SAMPLE entries are cut to the same seeded, sorted sample of positions every run.  Under torchrun only rank 0
+    writes, so the dual solution is that rank's block of constraint rows."""
+    os.makedirs(out_dir, exist_ok=True)
+
+    def sample(v, seed):
+        v = np.asarray(v, np.float64)
+        if v.size <= DUMP_SAMPLE:
+            return v
+        return v[np.sort(np.random.default_rng(seed).choice(v.size, DUMP_SAMPLE, replace=False))]
+
+    np.save(os.path.join(out_dir, "primal_solution.npy"), sample(x, 1))
+    np.save(os.path.join(out_dir, "dual_solution.npy"), sample(y, 2))
+    np.save(os.path.join(out_dir, "reduced_costs.npy"), sample(rc, 3))
+    np.save(os.path.join(out_dir, "objectives_and_iterations.npy"),
+            np.array([st.primal_objective, st.dual_objective, st.number_of_steps_taken], np.float64))
+
+
 def run_reference(args):
     """CPU arm: the reference's PDLP as restated by the oracle port, all host threads, bounded sample."""
     rank = int(os.environ.get("RANK", "0"))
@@ -267,7 +280,11 @@ def main():
                     help="seconds given to the reference's own CPU path (dual simplex, 1 core) on this LP; 0 = skip")
     ap.add_argument("--comparator", default="auto", choices=["auto", "off"],
                     help="time the cuSPARSE/cuBLAS re-assembly of the reference's attempt (scripts/cusparse_pdhg.cu) beside ours")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned as DIR/<name>.npy (float64; long vectors sampled)")
     args = ap.parse_args()
+    if args.dump_outputs and args.steps < 1:
+        ap.error("--dump-outputs writes what the last timed step returned: it needs --steps >= 1")
     if args.cpu_iters <= 0:  # the OpenMP oracle runs roughly 1e8 nonzeros/s of PDHG iteration on 8 cores
         nnz_guess = {"c4": 80e6, "c2": 8e6, "c3": 0.9e6}[args.workload]
         args.cpu_iters = int(max(4, min(400, 1.5e8 / nnz_guess * 4)))
@@ -302,8 +319,9 @@ def main():
         shard = shard[:2] + tuple(np.ascontiguousarray(a) for a in shard[2:])
 
     gsol_status = [None]
+    last_outputs = [None]  # (primal, dual, reduced costs, stats) of the latest one_step(keep=True)
 
-    def one_step():
+    def one_step(keep=False):
         # e2e path: HOST numpy buffers -> C ABI -> HOST result buffers
         if world == 1:
             p = capi.Problem.create_ranged(lp.offsets, lp.indices, lp.values, lp.con_lb, lp.con_ub, lp.c, lp.var_lb,
@@ -318,6 +336,8 @@ def main():
         x = sol.primal(); y = sol.dual()
         st = sol.stats()
         gsol_status[0] = sol.termination_reason
+        if keep:  # the dumped step only: no extra host copy of the reduced costs in any other timed step
+            last_outputs[0] = (x, y, sol.reduced_costs(), st)
         return st, float(x[0] + y[0])
 
     def barrier():
@@ -333,8 +353,8 @@ def main():
         sampler.start()
     t0 = time.perf_counter()
     its = 0; dev_s = 0.0; launches = 0; setup_s = 0.0; loop_s = 0.0; term_s = 0.0
-    for _ in range(args.steps):
-        st, _ = one_step()
+    for i in range(args.steps):
+        st, _ = one_step(keep=bool(args.dump_outputs) and i == args.steps - 1)
         its += st.number_of_steps_taken
         dev_s += st.pdhg_loop_seconds + st.termination_seconds
         loop_s += st.pdhg_loop_seconds; term_s += st.termination_seconds
@@ -343,6 +363,8 @@ def main():
     barrier()
     wall = time.perf_counter() - t0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *last_outputs[0])
 
     # max over ranks (device time and wall), sum of iterations
     if world > 1:
@@ -393,19 +415,15 @@ def main():
         launched_as = dom if blocks <= 1 else (
             f"{blocks - 1} x k_block_pass + {dom}<INIT> on the last column block (gather blocking: the step's product is split "
             "by column blocks, the row epilogue is fused into the last block's pass; timed as one group)")
-        # DRAM traffic of that step from the committed `ncu --set full` capture of the same workload (bytes per step)
-        traffic, traffic_src = NCU_TRAFFIC.get((args.workload, dom, blocks > 1), (None, None))
         roof = {"bound": "hbm", "kernel": dom, "launched_as": launched_as, "achieved": achieved, "peak": peaks["hbm_gbs"],
-                "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"], "traffic": traffic,
-                "traffic_source": None if traffic is None else f"committed capture: {traffic_src}",
-                "peak_source": peak_kind, "algorithmic_bytes_per_launch": by, "ms_per_launch": ms,
+                "unit": "GB/s", "frac": achieved / peaks["hbm_gbs"], "peak_source": peak_kind, "algorithmic_bytes_per_launch": by, "ms_per_launch": ms,
                 "measured_on": "1 GPU, the full LP" + ("" if world == 1 else
                                f" (a probe on rank 0's GPU beside the {world}-GPU run: the sharded attempt runs other kernels on 1/{world} of the rows; see detail.kernels)")}
-        # second bound of the SpMV steps (profiles/r2/request_port_roofline.md): every gathered double of a random column is one
-        # L1TEX miss request and an SM sends at most one request per clock towards L2
+        # second bound of the SpMV steps: every gathered double of a random column is one L1TEX miss request and an SM sends
+        # at most one request per clock towards L2
         try:
             sm_count = torch.cuda.get_device_properties(local).multi_processor_count
-            sm_hz = 1e6 * float((clocks or {}).get("sm_mhz") or (clocks or {}).get("sm_max_mhz") or 1965.0)
+            sm_hz = 1e6 * float((clocks or {}).get("sm_mhz") or (clocks or {}).get("sm_max_mhz") or 1980.0)
             floor_ms = 1e3 * (lp.nnz + (12 * lp.nnz) / 128.0) / (sm_count * sm_hz)  # gathers + coalesced 128-byte stream requests
             roof["request_port"] = {"what": "L1TEX -> crossbar requests: 1 per clock per SM; one per gathered double + one per 128 B of matrix stream",
                                     "floor_ms_per_launch": floor_ms, "frac_of_floor": floor_ms / ms if dom != "k_primal_step" else None}
@@ -451,7 +469,8 @@ def main():
         out = {"metric": METRIC, "value": its / dev_s, "unit": UNIT, "n_gpus": world, "steps": args.steps,
                "warmup": args.warmup, "ms_per_step": 1e3 * wall / args.steps, "higher_is_better": True,
                "scaling": "strong", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
-               "config": config_dict(args, lp, world), "clocks": clocks,
+               "config": config_dict(args, lp, world, torch.cuda.get_device_properties(local).L2_cache_size),
+               "device": torch.cuda.get_device_name(local), "clocks": clocks,
                "e2e": {"value": its / wall, "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
                "gpu_launches": launches, "roofline": roof, "cpu_baseline": cpu, "detail": extra}
         print(json.dumps(out))

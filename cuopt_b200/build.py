@@ -1,4 +1,4 @@
-"""Builds cuopt_b200/lib/libcuopt.so (sm_100a) with nvcc.  No JIT, no torch: the library is a plain C-ABI .so."""
+"""Builds cuopt_b200/lib/libcuopt.so (sm_90a) with nvcc.  No JIT, no torch: the library is a plain C-ABI .so."""
 from __future__ import annotations
 
 import os
@@ -42,7 +42,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         return LIB
     os.makedirs(LIB_DIR, exist_ok=True)
     host_cxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else None
-    cmd = [nvcc_path(), "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [nvcc_path(), "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "-Xcompiler", "-fPIC", "-shared", "-x", "cu",
            "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
     if host_cxx:
@@ -73,7 +73,7 @@ def build_cli(force: bool = False) -> str:
     if not force and os.path.exists(CLI) and os.path.getmtime(CLI) >= max(os.path.getmtime(src), os.path.getmtime(lib)):
         return CLI
     os.makedirs(os.path.dirname(CLI), exist_ok=True)
-    cmd = [nvcc_path(), "-O2", "-std=c++17", "-x", "cu", "-gencode", "arch=compute_100a,code=sm_100a",
+    cmd = [nvcc_path(), "-O2", "-std=c++17", "-x", "cu", "-gencode", "arch=compute_90a,code=sm_90a",
            "-I" + os.path.join(ROOT, "include"), src, "-o", CLI, "-L" + LIB_DIR, "-lcuopt",
            "-Xlinker", "-rpath,$ORIGIN/../lib", "-Xcompiler", "-pthread"]
     res = subprocess.run(cmd, capture_output=True, text=True)

@@ -874,6 +874,6 @@ cuopt_int_t cuOptB200ReadProblem(const char* filename, cuopt_int_t fixed_format,
   }
 }
 
-const char* cuOptB200Version(void) { return "cuopt-b200 0.1.0 sm_100a"; }
+const char* cuOptB200Version(void) { return "cuopt-b200 0.1.0 sm_90a"; }
 
 }  // extern "C"

@@ -16,7 +16,7 @@ namespace cuopt_b200 {
 // SM count of the device the calling thread is bound to (a rank of a multi-GPU solve is not on device 0)
 static int current_device_sms()
 {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   return sms;
 }

@@ -1,5 +1,5 @@
 // Small CUDA helpers for the PDLP solver: error checking, RAII device buffers,
-// deterministic block reductions and cache-hinted loads.  sm_100a only.
+// deterministic block reductions and cache-hinted loads.  sm_90a (Hopper).
 #pragma once
 
 #include "lp_problem.hpp"
@@ -116,7 +116,7 @@ class device_block_cache_t {
   };
   device_block_cache_t()
   {
-    cap_ = size_t(48) << 30;
+    cap_ = size_t(16) << 30;  // a fifth of an 80 GB H100: several configs[3] solves' arrays, room left for the caller
     if (const char* e = std::getenv("CUOPT_B200_DEVICE_CACHE_MB")) cap_ = (size_t)std::strtoull(e, nullptr, 10) << 20;
   }
   std::mutex mu_;
@@ -246,7 +246,7 @@ __device__ __forceinline__ double block_reduce(double v, double* scratch)
 }
 
 // L2 residency hints (createpolicy + ld/st ...L2::cache_hint).  At configs[3] sizes the vector an SpMV gathers from is
-// 80 MB: it only stays in the 126 MB L2 if the ~2 GB of read-once streams passing by are marked evict-first and
+// 80 MB: a large share of it only stays in L2 if the ~2 GB of read-once streams passing by are marked evict-first and
 // the vector itself evict-last.  `keep` marks the gathered vector (its producer's stores and the gathers), `stream`
 // everything that is touched once per kernel.  Mode 0 (CUOPT_B200_L2_HINTS=0) makes both policies evict-normal.
 struct l2_policy_t {

@@ -1,4 +1,4 @@
-// Hand-written sm_100a kernels of the PDLP hot path.
+// Hand-written sm_90a kernels of the PDLP hot path.
 //
 // One PDHG attempt = three launches (K1 primal step, K2 A*xbar + dual step,
 // K3 A^T*y' + interaction/movement reductions + step-size rule), replacing the
@@ -19,7 +19,7 @@
 // fixed grid, so results are bit-reproducible run to run.  For large LPs K2 / K3 are split by column blocks ("gather
 // blocking", further down) with the row epilogue fused into the LAST block's pass; the sharded multi-GPU attempt and its
 // NVLink peer transport follow the single-GPU kernels; the evaluation / infeasibility kernels are element-wise over
-// products formed by k_spmv.  DESIGN.md §5 has the measurements behind each of these choices.
+// products formed by k_spmv.  DESIGN.md §5 describes these choices and their measurements.
 #pragma once
 
 #include "device_utils.cuh"
@@ -30,7 +30,7 @@
 namespace cuopt_b200 {
 
 constexpr int EW_THREADS  = 256;  // element-wise kernels
-static __device__ int g_l2_hints = 1;  // device_utils.cuh make_l2_policies; CUOPT_B200_L2_HINTS=0 clears it (measured: profiles/r1/l2_hints_experiment.txt)
+static __device__ int g_l2_hints = 1;  // device_utils.cuh make_l2_policies; CUOPT_B200_L2_HINTS=0 clears it
 
 // Device-resident control block: every scalar the PDHG loop reads or writes.
 struct pdhg_ctl_t {
@@ -552,7 +552,7 @@ __global__ void __launch_bounds__(EW_THREADS) k_fill_list(int n, const int* __re
 // consumer, see pdlp_solver.cu enqueue_gather_attempt): for every destination rank, its slots in DESTINATION order — thread k
 // stores v[list[k]] into slot base + k, warps aligned to 256-byte segments of the destination, so the NVLink stores are
 // full contiguous lines (stores issued in SOURCE order by the producing kernel hit every destination with ragged ~20-of-32
-// lane runs and reached half the link rate: profiles/r2/dist_slot_trace_c4_n8_fused_stores.txt).  First halves of all
+// lane runs, which use the link far less efficiently than full lines).  First halves of all
 // destinations, flag A, second halves, flag B.  Destinations are visited starting after the sender's own rank.
 constexpr int SEND_UNROLL = 8;
 struct send_plan_t {
@@ -870,9 +870,8 @@ __global__ void k_step_rule_gather(pdhg_ctl_t* __restrict__ ctl, const double* _
 
 // ---------------------------------------------------------------------------------------------
 // Gather blocking (large LPs).  When the vector an SpMV gathers from is much larger than what stays in L2 (80 MB at
-// configs[3] against a 126 MB L2 that also sees ~2 GB of streams per kernel), ncu shows the fused kernels DRAM-bound
-// at 2.4x their algorithmic bytes: every gathered double drags a 32-byte sector in from HBM (profiles/r1).  The
-// host then splits the matrix by COLUMN blocks whose slice of the gathered vector is L2-sized (csr_transpose.cu),
+// configs[3], against an L2 that also sees ~2 GB of streams per kernel), the fused kernels turn DRAM-bound well above
+// their algorithmic bytes: every gathered double drags a 32-byte sector in from HBM.  The host then splits the matrix by COLUMN blocks whose slice of the gathered vector is L2-sized (csr_transpose.cu),
 // and K2 / K3 become   (B - 1) x k_block_pass (t += A_b * x, payload-free)  +  the fused kernel on the LAST block with
 // INIT = true (its row sums start from t, its row epilogue is the step's).  Rows keep their entry order inside and across
 // blocks; the result is t_0 + t_1 + ... in block order.

@@ -1,4 +1,4 @@
-// B200-native PDLP driver: device data layout, setup (transpose, diagonal scaling), the
+// H100-native PDLP driver: device data layout, setup (transpose, diagonal scaling), the
 // batched PDHG loop and the major-iteration logic (termination test + KKT restart).
 //
 // Control flow follows pdlp_solver_t::run_solver (cpp/src/linear_programming/pdlp.cu:984-1185)
@@ -311,6 +311,12 @@ void upload_csr(csr_dev_t& d, int rows, int cols, const VI& off, const VI& idx, 
   build_bicsr(d, off, s, sms);
 }
 
+// Gather blocking (pdlp_kernels.cuh): the largest slice of the gathered vector one column block may span, as a share of the
+// device's L2.  Every extra block costs one more read and write of the row sums, so blocks stay as wide as the cache allows.
+// configs[3] on an H100 80GB HBM3 (400 W power limit, 50 MB L2), PDLP iterations/s: 16 MB blocks (this fraction) 312,
+// 24 MB 311, 40 MB 232, unblocked 184.
+constexpr double GATHER_BLOCK_L2_FRACTION = 0.32;
+
 }  // namespace
 
 struct pdlp_solver_t::impl_t {
@@ -321,7 +327,7 @@ struct pdlp_solver_t::impl_t {
   pdlp_hyper_params_t hp;
   pdlp_settings_t st;
   cudaStream_t stream = nullptr;
-  int sms             = 148;
+  int sms             = 132;
 
   csr_dev_t A, AT, As, ATs;
   dvec<double> c, l, u, lc, uc, cs, ls, us, lcs, ucs, Dr, Dc;
@@ -355,11 +361,10 @@ struct pdlp_solver_t::impl_t {
   int cntX = 0, cntY = 0;    // packed lengths (second half starts at half the length)
   bool dist_pack = true;     // CUOPT_B200_DIST_PACK=0: identity packing (everything travels), for comparison
   // How the packed entries travel.  "fused" (default): the producing kernels (K1, K2) issue the peer stores themselves, in
-  // source order, overlapped with their own work: 588 us per attempt at configs[3] on 2 GPUs, 363 us on 8 (measured).
+  // source order, overlapped with their own work.
   // "kernel" (CUOPT_B200_DIST_SEND=kernel): k_send_packed on a second stream, destination order (full 256-byte lines), halves
-  // pipelined with the consumer's column blocks.  Measured on 2 GPUs only: 790 us per attempt — the SpMV kernels lose the CTA
-  // slots reserved for the send kernel and the first half's wire time is exposed; the 8-GPU regime it was written for (wire-
-  // bound attempts, source-order stores at half the link rate) could not be measured inside this round's GPU budget.
+  // pipelined with the consumer's column blocks.  The SpMV kernels lose the CTA slots reserved for the send kernel, so it
+  // only pays where the attempt is wire-bound (many ranks, ragged source-order stores); opt-in, speed not measured on H100.
   bool dist_send_kernel = false;
   cudaStream_t comm_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -428,7 +433,7 @@ struct pdlp_solver_t::impl_t {
   };
   gather_blocks_t blkA, blkAT, blkATslice;
   dvec<double> t_m, t_n;
-  size_t gather_block_bytes = 40u << 20;  // measured optimum at configs[3] (profiles/r1/gather_block_sweep_c4.txt)
+  size_t gather_block_bytes = 0;  // set in build() from the device's L2 size (see there)
   int n_part_dy2 = 1;  // CTAs that publish ||dy||^2 partials: grid_k2 (fused K2) or grid_m (blocked K2 epilogue)
   int grid_k1 = 1, grid_k2 = 1, grid_k3 = 1, grid_n = 1, grid_m = 1, grid_misc = 1;
   std::map<int, cudaGraphExec_t> graphs;
@@ -644,7 +649,13 @@ struct pdlp_solver_t::impl_t {
     grid_misc = ew_grid(std::max(n, m), sms);
     part_dy2.resize((size_t)std::max({grid_k2, grid_m, sms * 16}));
     n_part_dy2 = grid_k2;
-    // size of the slice of the gathered vector one column block may span (0 = never block); bytes, for the tests too
+    // size of the slice of the gathered vector one column block may span (0 = never block); bytes, for the tests too.
+    // GATHER_BLOCK_L2_FRACTION of the L2: the slice shares the cache with the matrix streams and the row sums passing by
+    {
+      int l2 = 0;
+      CUOPT_CUDA_TRY(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
+      gather_block_bytes = (size_t)((double)l2 * GATHER_BLOCK_L2_FRACTION);
+    }
     if (const char* e = std::getenv("CUOPT_B200_GATHER_BLOCK_BYTES")) gather_block_bytes = (size_t)std::atoll(e);
     part_k3.resize(2 * (size_t)std::max({grid_k3, grid_n, sms * 16}));
     part_rows.resize(6 * (size_t)grid_m);
@@ -758,7 +769,7 @@ struct pdlp_solver_t::impl_t {
       CUOPT_CUDA_TRY(cudaStreamCreateWithFlags(&comm_stream, cudaStreamNonBlocking));
       CUOPT_CUDA_TRY(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
       CUOPT_CUDA_TRY(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-      send_slots = sms;  // measured on 2 GPUs: 32 slots / 64 send CTAs cannot feed the link (880 us per attempt against 790)
+      send_slots = sms;  // one slot per SM: far fewer send CTAs cannot keep the link busy
       if (const char* e = std::getenv("CUOPT_B200_DIST_SEND_SLOTS")) send_slots = std::max(1, std::min(std::atoi(e), sms));
       grid_send = 2 * send_slots;
     }
@@ -1260,7 +1271,7 @@ struct pdlp_solver_t::impl_t {
   {
     const bool blocked = blkAT.on();
     const csr_dev_t& L = blocked ? blkAT.blk[blkAT.B - 1] : ATs;
-    const int npre     = npre_override > 1 ? 2 : 1;  // measured at configs[3]: two payload sets pay in K2 (-20 us), not here (+19 us)
+    const int npre     = npre_override > 1 ? 2 : 1;  // two payload sets pay in K2 only (fused_npre), not in this last pass
     const int grid     = spmv_grid(L, npre);
     const double* t    = blocked ? t_n.data() : nullptr;
     if (blocked) launch_block_passes(blkAT, blkAT.B - 1, ybuf[0].data(), ybuf[1].data(), 1, t_n.data(), nullptr, 0);

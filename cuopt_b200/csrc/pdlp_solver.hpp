@@ -1,4 +1,4 @@
-// Host-visible interface of the B200 PDLP solver (no CUDA types: c_api.cpp includes this).
+// Host-visible interface of the PDLP solver (no CUDA types: c_api.cpp includes this).
 //
 // Counterpart of the reference's pdlp_solver_t / solve_lp
 // (cpp/src/linear_programming/pdlp.cuh, solve.cu:554-613) for the PDLP method.

@@ -1,4 +1,4 @@
-// Block-interleaved CSR ("BICSR"): the storage format and SpMV core of every sparse product of the solver (sm_100a).
+// Block-interleaved CSR ("BICSR"): the storage format and SpMV core of every sparse product of the solver (sm_90a).
 //
 // Layout.  The host cuts the rows of a CSR matrix into blocks of whole consecutive rows with at most 256 entries and at
 // most 256 rows.  Block b owns the 256 slots [256 b, 256 b + 256) of the index / value arrays; slot 32 k + l holds the
@@ -19,8 +19,8 @@
 //   4. ONE double per row goes through shared memory — written to the slot of the row's last entry, read by the lane that
 //      runs the row epilogue (lane r mod 32 of row r, so the epilogue's vector accesses are coalesced).
 // Against the round-1 core (products parked in shared memory, one lane per row re-reading them) this removes ~80 % of the
-// shared-memory wavefronts and every per-entry bank conflict from the L1TEX unit that also has to serve the gathers;
-// measured on the bench matrices it is 5-12 % faster per pass (profiles/r2/spmv_lab_uniform.txt).
+// shared-memory wavefronts and every per-entry bank conflict from the L1TEX unit that also has to serve the gathers
+// (scripts/spmv_lab.cu compares the two).
 //
 // Summation order.  Inside a lane: strictly left to right.  A row that spans lanes is (carry from the earlier lanes) +
 // (this lane's left-to-right part).  Everything is a fixed function of the block cut, so results are bit-reproducible run

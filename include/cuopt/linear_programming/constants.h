@@ -1,5 +1,5 @@
 /*
- * Drop-in ABI constants for the libcuopt LP C interface (B200-native PDLP build).
+ * Drop-in ABI constants for the libcuopt LP C interface (H100-native PDLP build).
  *
  * The numeric values and parameter-name strings below are the wire contract of
  * the reference header cpp/include/cuopt/linear_programming/constants.h:26-113

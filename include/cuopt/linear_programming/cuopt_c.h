@@ -1,5 +1,5 @@
 /*
- * libcuopt LP C interface — B200-native PDLP build.
+ * libcuopt LP C interface — H100-native (sm_90a) PDLP build.
  *
  * This header declares, with identical names, argument order, scalar types and
  * status codes, the 41 entry points of the reference C API
@@ -9,7 +9,7 @@
  * against the reference header can be relinked against this library.
  *
  * Scope: LP only, solved by PDLP on one (or, through the cuopt_b200_ext.h
- * extension, several) B200 GPUs.  A problem that declares integer variables
+ * extension, several) H100 GPUs.  A problem that declares integer variables
  * is reported by cuOptIsMIP, and cuOptSolve answers it with an error solution
  * (CUOPT_VALIDATION_ERROR) instead of running a MIP search.
  *

@@ -1,5 +1,5 @@
 /*
- * Extension entry points of the B200-native libcuopt LP build.
+ * Extension entry points of the H100-native libcuopt LP build.
  *
  * The reference C ABI (cuopt_c.h) has no way to read the iteration count, the dual objective or the
  * residuals of an LP solve: they live in additional_termination_information_t
@@ -148,7 +148,7 @@ cuopt_int_t cuOptB200WarmStartGetVector(cuOptB200WarmStart warm_start,
  * its C++ parse_mps(file, fixed_mps_format) has the flag: cpp/libmps_parser/include/mps_parser/parser.hpp:33). */
 cuopt_int_t cuOptB200ReadProblem(const char* filename, cuopt_int_t fixed_format, cuOptOptimizationProblem* problem_ptr);
 
-/* Library identification: "cuopt-b200 <version> sm_100a". */
+/* Library identification: "cuopt-b200 <version> sm_90a". */
 const char* cuOptB200Version(void);
 
 #ifdef __cplusplus

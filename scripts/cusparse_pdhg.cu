@@ -16,7 +16,7 @@
 // captured in one CUDA graph per attempt like the reference does; the per-attempt host synchronisation the reference
 // needs is reported separately (with and without).
 //
-// nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -Xcompiler -fopenmp scripts/cusparse_pdhg.cu -lcusparse -lcublas -o scripts/_bin/cusparse_pdhg   (python -c "import __graft_entry__ as g; g.build_tools()")
+// nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -Xcompiler -fopenmp scripts/cusparse_pdhg.cu -lcusparse -lcublas -o scripts/_bin/cusparse_pdhg   (python -c "import __graft_entry__ as g; g.build_tools()")
 #include <cublas_v2.h>
 #include <cuda_runtime.h>
 #include <cusparse.h>
@@ -176,7 +176,7 @@ int main(int argc, char** argv)
   std::vector<int> sizes;
   for (int i = 1; i < argc; ++i) sizes.push_back(atoi(argv[i]));
   if (sizes.empty()) sizes = {1000000, 10000000};
-  int sms = 148;
+  int sms = 0;
   CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   cudaStream_t stream, s1, s2;
   CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));

@@ -1,11 +1,11 @@
-// CTA-staged / warp-consumed CSR row blocks (sm_100a): TMA takes the matrix stream off the L1TEX request path.
+// CTA-staged / warp-consumed CSR row blocks (sm_90a: TMA bulk copies + mbarrier): TMA takes the matrix stream off the L1TEX request path.
 //
 // ncu on the plain warp-synchronous kernels (spmv_warp.cuh) shows they execute in exactly
 // l1tex__t_sectors / #SM cycles: ~1 global-load sector per clock per SM, of which 8.0 M are the unavoidable
 // gathers, 3.0 M the (col,val) stream and ~1.4 M epilogue operands.  Here the (col,val,row-offset) slices of a
 // GROUP of 8 consecutive warp blocks (<= 2048 nonzeros, one contiguous range) are fetched by ONE producer warp with
 // three cp.async.bulk copies per group (bulk copies must be large: per-warp 1-2 KB copies ran at ~95 cycles per
-// copy and made the kernels 2x slower, profiles/r1), land in shared memory through the TMA unit, and are consumed by
+// copy and made the kernels slower), land in shared memory through the TMA unit, and are consumed by
 // 8 independent consumer warps, one warp block each, exactly as in spmv_warp.cuh: 8 gathers per lane, products
 // parked in place (XOR-swizzled), left-to-right row sums, fused epilogue.  Synchronisation is by mbarriers only
 // (full[stage]: producer -> consumers, transaction count; empty[stage]: 8 consumer arrivals -> producer); there is no

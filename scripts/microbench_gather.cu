@@ -1,8 +1,8 @@
-// Micro-benchmarks that bound the SpMV design on B200 (run under gpurun; results quoted in DESIGN.md):
+// Micro-benchmarks that bound the SpMV design on the GPU:
 //   1. streaming read of a 96 MB + 64 MB (idx,val) pair        -> achievable HBM rate for the matrix stream
 //   2. random 8-byte gathers from an 8 MB / 80 MB fp64 vector   -> L2 / HBM sector-gather rate (32 B per gather)
 //   3. stream + gather together (the SpMV access pattern without any reduction)
-// nvcc -O3 -gencode arch=compute_100a,code=sm_100a scripts/microbench_gather.cu -o gpurun_out/microbench_gather
+// nvcc -O3 -gencode arch=compute_90a,code=sm_90a scripts/microbench_gather.cu -o microbench_gather
 #include <cuda_runtime.h>
 
 #include <cstdio>

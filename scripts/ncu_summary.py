@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (captured with `ncu --set full`) into a small markdown table for profiles/.
-usage: python scripts/ncu_summary.py gpurun_out/prof.ncu-rep > profiles/rNN/xxx.md"""
+"""Summarise an .ncu-rep (captured with `ncu --set full`) into a small markdown table.
+usage: python scripts/ncu_summary.py prof.ncu-rep > summary.md"""
 import csv
 import subprocess
 import sys

@@ -1,7 +1,7 @@
 // NVLink peer-store microbenchmark (measurement tool, not the product): how fast can SM-issued stores / the copy engines
 // move a vector slice into a peer GPU's memory?  One process, all visible devices; every device stores into the NEXT one
 // at the same time (the bidirectional pattern of the sharded PDHG attempt).
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a scripts/nvlink_store_bench.cu -o scripts/_bin/nvlink_store_bench
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a scripts/nvlink_store_bench.cu -o scripts/_bin/nvlink_store_bench
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdlib>
@@ -41,6 +41,8 @@ int main(int argc, char** argv)
 {
   int nd = 0;
   CK(cudaGetDeviceCount(&nd));
+  int sms = 0;  // grids are multiples of the SM count
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
   if (nd < 2) { std::printf("needs >= 2 devices\n"); return 0; }
   const size_t n = argc > 1 ? std::strtoull(argv[1], nullptr, 10) : 5000000;  // doubles per transfer
   std::vector<double*> src(nd), dst(nd), aux(nd);
@@ -68,7 +70,7 @@ int main(int argc, char** argv)
   };
   std::printf("%d devices, %zu doubles (%.1f MB) per transfer\n", nd, n, n * 8 / 1e6);
   for (int dirs : {1, nd}) {
-    for (int grid : {148 * 4, 148 * 8, 148 * 16}) {
+    for (int grid : {sms * 4, sms * 8, sms * 16}) {
       char nm[128];
       std::snprintf(nm, sizeof nm, "SM stores  8 B/thread, grid %4d x 256", grid);
       run(nm, dirs, [&](int d) { k_store8<<<grid, 256, 0, st[d]>>>(src[d], dst[(d + 1) % nd], n); });
@@ -78,17 +80,17 @@ int main(int argc, char** argv)
     run("copy engine (cudaMemcpyPeerAsync)", dirs, [&](int d) { CK(cudaMemcpyPeerAsync(dst[(d + 1) % nd], (d + 1) % nd, src[d], d, n * 8, st[d])); });
     run("local only: primal-like kernel, no remote store", dirs, [&](int d) {
       double* a = aux[d];
-      k_primal_like<<<148 * 8, 256, 0, st[d]>>>(a, a + n, a + 2 * n, a + 3 * n, a + 4 * n, a + 5 * n, a + 6 * n, nullptr, n); });
+      k_primal_like<<<sms * 8, 256, 0, st[d]>>>(a, a + n, a + 2 * n, a + 3 * n, a + 4 * n, a + 5 * n, a + 6 * n, nullptr, n); });
     run("primal-like kernel + remote store of xbar", dirs, [&](int d) {
       double* a = aux[d];
-      k_primal_like<<<148 * 8, 256, 0, st[d]>>>(a, a + n, a + 2 * n, a + 3 * n, a + 4 * n, a + 5 * n, a + 6 * n, dst[(d + 1) % nd], n); });
+      k_primal_like<<<sms * 8, 256, 0, st[d]>>>(a, a + n, a + 2 * n, a + 3 * n, a + 4 * n, a + 5 * n, a + 6 * n, dst[(d + 1) % nd], n); });
   }
   // fan-out: device 0 stores the same slice into EVERY other device (the all-gather pattern at nd ranks), everyone at once
   if (nd > 2) {
     std::printf("fan-out: every device stores its slice into all %d peers (egress = %d x slice)\n", nd - 1, nd - 1);
     const size_t ns = n / nd;
     run("SM stores 8 B/thread to all peers (GB/s = egress of one device)", nd, [&](int d) {
-      for (int p = 1; p < nd; ++p) k_store8<<<148 * 2, 256, 0, st[d]>>>(src[d], dst[(d + p) % nd] + (size_t)d * ns, ns); }, ns * 8 * (nd - 1));
+      for (int p = 1; p < nd; ++p) k_store8<<<sms * 2, 256, 0, st[d]>>>(src[d], dst[(d + p) % nd] + (size_t)d * ns, ns); }, ns * 8 * (nd - 1));
   }
   return 0;
 }

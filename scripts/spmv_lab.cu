@@ -1,6 +1,6 @@
-// SpMV laboratory, round 2 (run under gpurun; results summarised in profiles/r2/).
+// SpMV laboratory.
 //
-// Question: what does a row-structured fp64 CSR SpMV with uniformly random columns cost on a B200 at the sizes of
+// Question: what does a row-structured fp64 CSR SpMV with uniformly random columns cost on the GPU at the sizes of
 // BASELINE.json's configs[1] / configs[3], and how close can a kernel get to the rowless "stream + gather" ceiling?
 // Candidates (all verified against a thread-per-row reference before they are timed):
 //   base<RPL>     the round-1 production core (spmv_warp.cuh): coalesced loads, products parked in shared memory,
@@ -11,7 +11,7 @@
 //                 sums of rows that cross lanes are chained by shuffles, and only ONE double per row goes through shared
 //                 memory (slot of the row's last entry) to reach the lane that runs the row epilogue.
 //   gather<U>, stream_gather<U>   rowless ceilings (no reduction at all)
-// nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a -lineinfo -Icuopt_b200/csrc -Iinclude scripts/spmv_lab.cu -o gpurun_out/spmv_lab
+// nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a -lineinfo -Icuopt_b200/csrc -Iinclude scripts/spmv_lab.cu -o scripts/_bin/spmv_lab
 #include "pdlp_kernels.cuh"
 
 // ---- the round-1 core (spmv_warp.cuh of round 1), kept here as the baseline the new format is measured against ----
@@ -514,7 +514,7 @@ __global__ void k_warm(const double* __restrict__ x, size_t count)
 static int g_mode               = 0;  // 0 hot (back-to-back repetitions), 1 cold (L2 flushed before every repetition), 2 cold, L2 full of stale evict-last lines
 static double* g_flush   = nullptr;
 static size_t g_flush_n  = 0;
-static int g_sms         = 148;
+static int g_sms         = 0;
 static bool g_need_flush = false;
 
 template <typename F>

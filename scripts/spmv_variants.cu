@@ -1,6 +1,6 @@
-// Stand-alone exploration of SpMV kernel shapes for configs[1] (1M x 1M, 8 nnz/row, random columns) on B200.
+// Stand-alone exploration of SpMV kernel shapes for configs[1] (1M x 1M, 8 nnz/row, random columns).
 // y = A x only (no PDHG epilogue).  Prints microseconds per SpMV for each variant; results feed DESIGN.md.
-// nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a scripts/spmv_variants.cu -o /tmp/spmv_variants
+// nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a scripts/spmv_variants.cu -o /tmp/spmv_variants
 #include <cuda_runtime.h>
 
 #include <cstdint>

@@ -1,5 +1,5 @@
-// Exploration: warp-synchronous row blocks (no __syncthreads, 2048 threads/SM) for configs[1] on B200.
-// nvcc -O3 -std=c++17 -gencode arch=compute_100a,code=sm_100a scripts/spmv_warp_rows.cu -o /tmp/swr
+// Exploration: warp-synchronous row blocks (no __syncthreads, 2048 threads/SM) for configs[1].
+// nvcc -O3 -std=c++17 -gencode arch=compute_90a,code=sm_90a scripts/spmv_warp_rows.cu -o /tmp/swr
 #include <cuda_runtime.h>
 
 #include <algorithm>

@@ -1,7 +1,10 @@
+import atexit
 import gzip
 import json
 import os
+import shutil
 import sys
+import tempfile
 
 import numpy as np
 import pytest
@@ -15,7 +18,7 @@ MPS_DIR = os.path.join(GOLDEN, "mps")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: pytest -m gpu)")
     config.addinivalue_line("markers", "slow: larger sizes")
 
 
@@ -26,14 +29,26 @@ def mps_path(rel: str, tmp_dir=None) -> str:
         return p
     gz = p + ".gz"
     if os.path.exists(gz):
-        out_dir = tmp_dir or os.path.join(ROOT, "gpurun_out", "_tmp")
+        out_dir = tmp_dir or _session_dir()
         os.makedirs(out_dir, exist_ok=True)
-        out = os.path.join(out_dir, os.path.basename(p))
+        out = os.path.join(out_dir, rel.replace("/", "__"))  # the whole relative path: no two fixtures share a name
         if not os.path.exists(out):
             with open(out, "wb") as f:
                 f.write(gzip.open(gz).read())
         return out
     raise FileNotFoundError(rel)
+
+
+_SESSION_DIR = []
+
+
+def _session_dir() -> str:
+    """A private directory for this test session, removed when it ends: nothing inflated by an earlier run is reused."""
+    if not _SESSION_DIR:
+        d = tempfile.mkdtemp(prefix="cuopt_b200_mps_")
+        atexit.register(shutil.rmtree, d, True)
+        _SESSION_DIR.append(d)
+    return _SESSION_DIR[0]
 
 
 def load_golden(name: str):

@@ -30,7 +30,7 @@ def test_library_loads_and_exports_every_declared_symbol():
         declared |= set(re.findall(r"\b(cuOpt[A-Za-z0-9]+)\s*\(", text))
     assert declared == set(capi.REFERENCE_SYMBOLS + capi.EXTENSION_SYMBOLS)
     assert len(capi.REFERENCE_SYMBOLS) == 41
-    assert b"sm_100a" in L.cuOptB200Version()
+    assert b"sm_90a" in L.cuOptB200Version()
 
 
 def test_scalar_sizes():

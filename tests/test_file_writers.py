@@ -1,12 +1,14 @@
 """`user_problem_file` / `solution_file` (constants.h parameter names; the reference's solve_lp writes them around the
 solve, cpp/src/linear_programming/solve.cu:586-601).  The MPS writer restates cpp/src/mip/problem/write_mps.cu; what it
-writes is read back by this repo's reader AND by the reference's own libmps_parser (oracle/_ref)."""
+writes is read back by this repo's reader AND by the reference's own libmps_parser (oracle/_ref, or what it read as stored
+in tests/golden/writer_golden.json)."""
+import hashlib
 import os
 
 import numpy as np
 import pytest
 
-from conftest import mps_path, problem_arrays
+from conftest import load_golden, mps_path, problem_arrays
 from cuopt_b200 import capi, lpgen
 
 
@@ -45,14 +47,43 @@ def test_written_mps_reads_back_identically(tmp_path, rel):
     assert a["maximize"] == b["maximize"] and p.is_mip == q.is_mip
 
 
+def canonical_digests(offsets, indices, values, m, n, **vectors) -> dict:
+    """sha256 prefixes of A as sorted CSR (independent of the entry order inside rows) and of the given vectors."""
+    import scipy.sparse as sp
+
+    def digest(a):
+        return hashlib.sha256(np.ascontiguousarray(a).tobytes()).hexdigest()[:16]
+    A = sp.csr_matrix((np.asarray(values, np.float64), np.asarray(indices, np.int32), np.asarray(offsets, np.int32)),
+                      shape=(m, n))
+    A.sort_indices()
+    out = dict(offsets=digest(A.indptr.astype(np.int32)), indices=digest(A.indices.astype(np.int32)),
+               values=digest(A.data.astype(np.float64)))
+    out.update({k: digest(np.asarray(v, np.float64)) for k, v in vectors.items()})
+    return out
+
+
+def WRITER_LP():
+    return lpgen.sparse_lp(300, 250, 5, seed=3)   # E / L / G rows, x >= 0
+
+
 def test_reference_parser_reads_what_we_write(tmp_path):
+    """Where oracle/_ref is built, the reference's parser reads the written file live; everywhere, the file must be the one
+    the reference's parser read when tests/golden/writer_golden.json was made (scripts/gen_golden_writer.py), and what it
+    read then must be this LP."""
     from oracle import ref_cpu
-    if not ref_cpu.available():
-        pytest.skip("oracle/_ref not built")
-    lp = lpgen.sparse_lp(300, 250, 5, seed=3)   # E / L / G rows, x >= 0
+    gold = load_golden("writer_golden.json")
+    lp = WRITER_LP()
     p = capi.Problem.create_ranged(lp.offsets, lp.indices, lp.values, lp.con_lb, lp.con_ub, lp.c, lp.var_lb, lp.var_ub)
     out = str(tmp_path / "written.mps")
     write_via_solve(p, out)
+    with open(out, "rb") as f:
+        assert hashlib.sha256(f.read()).hexdigest() == gold["written_mps_sha256"]
+    want = canonical_digests(lp.offsets, lp.indices, lp.values, lp.m, lp.n, c=lp.c, con_lb=lp.con_lb, con_ub=lp.con_ub,
+                             var_lb=lp.var_lb, var_ub=lp.var_ub)
+    assert (gold["reference_parse"]["m"], gold["reference_parse"]["n"]) == (lp.m, lp.n)
+    assert gold["reference_parse"]["digests"] == want
+    if not ref_cpu.available():
+        return
     m = ref_cpu.parse_mps(out)
     import scipy.sparse as sp
     A = sp.csr_matrix((lp.values, lp.indices, lp.offsets), shape=(lp.m, lp.n))

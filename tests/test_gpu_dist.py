@@ -1,5 +1,5 @@
 """Row-sharded multi-GPU solve (cuOptB200SolveDistributed) against the single-GPU solve of the same LP.
-Needs >= 2 GPUs (gpurun --gpus 2); skipped otherwise."""
+Needs >= 2 GPUs; skipped otherwise."""
 import os
 import socket
 
@@ -105,8 +105,8 @@ def test_sharded_iterates_track_the_single_gpu_iterates(transport, nnz_per_row):
     assert res[0]["its"] == one.stats().number_of_steps_taken == its
     x1, y1 = one.primal(), one.dual()
     y = np.concatenate([r["y"] for r in res])
-    # fp64 tolerance: 1e-7 of the largest entry after 120 iterations and their restarts (measured on the B200: 2e-9 for every
-    # transport — rounding differences of the row sums, amplified by the iteration; DESIGN.md section 3 uses the same bound
+    # fp64 tolerance: 1e-7 of the largest entry after 120 iterations and their restarts (rounding differences of the
+    # row sums, amplified by the iteration; DESIGN.md section 3 uses the same bound
     # for 120-iteration trajectories against the oracle)
     scale_x, scale_y = np.abs(x1).max(), np.abs(y1).max()
     assert np.abs(res[0]["x"] - x1).max() <= 1e-7 * scale_x
@@ -129,17 +129,16 @@ def test_two_gpu_solve_matches_single_gpu(mode, transport):
     assert res[0]["status"] == 1
     # agrees with the single-GPU run: objective to 1e-5 (planted optimum known; both stop at tolerance 1e-6),
     # the iteration count only loosely: partial sums are added in a different order, and at 1e-6 on this degenerate LP
-    # the restart decisions amplify last-bit differences (measured: 18 360 .. 21 200 against 19 400 on one GPU,
-    # 19 228 .. 29 640 against 27 512 in Fast1; scripts/dist_iteration_table.py)
+    # the restart decisions amplify last-bit differences (scripts/dist_iteration_table.py tabulates the counts)
     assert res[0]["obj"] == pytest.approx(lp.optimal_objective, rel=1e-5)
     assert res[0]["obj"] == pytest.approx(st1.primal_objective, rel=1e-5)
     assert res[0]["dobj"] == pytest.approx(st1.dual_objective, rel=1e-5)
-    # (round 2: 9 000 iterations with the gather transport against 17 440 on one GPU — the iterates agree to 2e-9 after 120
-    # iterations, test_sharded_iterates_track_the_single_gpu_iterates, and then part ways at a restart decision)
+    # (the iterates track the single-GPU ones through the first 120 iterations, test_sharded_iterates_track_the_single_gpu_iterates,
+    # and then part ways at a restart decision, so the count is only banded)
     assert 0.4 * st1.number_of_steps_taken <= res[0]["its"] <= 2.5 * st1.number_of_steps_taken
     # the dual blocks tile the dual vector.  The vectors themselves are NOT compared with the single-GPU ones: the
     # planted LP is degenerate (half of x* sits on its bound), its optimal dual face is not a point, and two
-    # tolerance-1e-6 runs land on it 17 % apart in norm (measured) while agreeing on both objectives to 1e-5.
+    # tolerance-1e-6 runs can land on it far apart in norm while agreeing on both objectives to 1e-5.
     y = np.concatenate([r["y"] for r in res])
     assert y.shape[0] == lp.m
     assert res[0]["rp"] <= 1e-6 * (1.0 + np.linalg.norm(np.where(np.isfinite(lp.con_ub), lp.con_ub, lp.con_lb))) * 10
@@ -148,7 +147,7 @@ def test_two_gpu_solve_matches_single_gpu(mode, transport):
 @pytest.mark.parametrize("world", [4, 8])
 def test_four_and_eight_gpu_solve_matches_single_gpu(world):
     """The same comparison on 4 and 8 ranks (peer-store transport; slices of 1/4 and 1/8 of the columns, rank-ordered sums of
-    4 / 8 partials): run with gpurun --gpus 4 / 8, skipped on smaller boxes."""
+    4 / 8 partials): needs 4 / 8 GPUs, skipped on smaller machines."""
     import torch
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")

@@ -197,7 +197,7 @@ def test_full_solve_vs_reference_simplex_and_oracle(simplex_golden, rel, tol, ot
                   maximize=a["maximize"], objective_offset=a["objective_offset"], tol=tol, iteration_limit=400000)
     r = o.solve()
     assert r["status"] == "Optimal"
-    # iteration counts: identical on most instances (see profiles/iteration_parity_r1.md); the two degenerate MIP
+    # iteration counts: identical on most instances; the two degenerate MIP
     # relaxations (50v-10, neos5) drift chaotically at deep tolerances: summation order flips a restart decision
     band = 0.30 if rel in ("mip/50v-10-free-bound.mps", "mip/neos5-free-bound.mps") else 0.0
     assert abs(st.number_of_steps_taken - r["iterations"]) <= max(40, band * r["iterations"])
@@ -313,7 +313,7 @@ def test_blocked_kernels_follow_the_oracle_step_by_step(forced_blocks, mode):
 
 def test_blocked_and_fused_paths_solve_identically(forced_blocks, monkeypatch):
     """Fused kernels vs gather-blocked passes (+ fused last pass) on the same LP, solved to 1e-8: the same optimum to 1e-6 in
-    the objective (round-1 finding: at tolerance 1e-6 two such runs are 1e-4 apart, which says nothing; at 1e-8 the bound
+    the objective (at tolerance 1e-6 two such runs can differ by far more than 1e-6, which says nothing; at 1e-8 the bound
     holds).  Iteration counts still react to last-bit differences through the restart decisions."""
     for lp in (lpgen.sparse_lp(3000, 2500, 6, seed=11), lpgen.multicommodity(60, 200, 4, seed=2)):
         p = lp_problem(lp)
@@ -346,5 +346,5 @@ def test_pds_shaped_config2_against_reference_dual_simplex():
         sol = capi.solve(lp_problem(lp), s)
         assert sol.termination_status == 1
         st = sol.stats()
-        assert st.primal_objective == pytest.approx(case["objective"], rel=1e-4)   # measured on the largest: 4.6e-7
+        assert st.primal_objective == pytest.approx(case["objective"], rel=1e-4)
         assert st.dual_objective == pytest.approx(case["objective"], rel=1e-4)

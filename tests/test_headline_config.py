@@ -5,8 +5,8 @@ headline 10M x 10M LP):
     fused last pass, device-side step rule — stepped against the OpenMP oracle element-wise from the same start;
   * configs[1] (1M x 1M) and configs[3]: solved through the C ABI until BOTH objectives are within 1e-6 relative of the
     planted optimum (north star: "converging to the reference's primal/dual objective within 1e-6 relative").  The PDLP
-    criteria are relative to 1 + |objective|, ||b||, ||c||: at tolerance 1e-6 the objectives of these LPs are still 5e-6 off
-    (measured), so the solves run at the tolerance given below.
+    criteria are relative to 1 + |objective|, ||b||, ||c||: at tolerance 1e-6 the objectives of these LPs are still a few 1e-6
+    off, so the solves run at the tolerance given below.
 
 fp64 tolerances: ELEMENTWISE 1e-11 relative to the vector's largest entry after identical steps (summation order inside a
 row: lanes / column blocks; reductions over 10M elements); scalars 1e-9."""
@@ -21,8 +21,7 @@ from test_gpu_parity import lp_problem, rel_err
 
 pytestmark = [pytest.mark.gpu, pytest.mark.slow]
 
-# tolerance at which PDLP's relative criteria imply 1e-6 on the objectives of the planted LPs (measured on the B200:
-# gpurun_out r2j; iterations / seconds in DESIGN.md §3)
+# tolerance at which PDLP's relative criteria imply 1e-6 on the objectives of the planted LPs (measured)
 TIGHT = 1e-7
 
 
@@ -73,15 +72,13 @@ def solve_to_planted_optimum(size, tolerance, objective_rel, time_limit):
 
 
 def test_config1_converges_to_the_planted_optimum_within_1e6():
-    # measured on the B200: Optimal after 227 600 iterations / 24 s; objectives 4.3e-7 (primal) and 5.0e-7 (dual) off
     solve_to_planted_optimum(1_000_000, TIGHT, 1e-6, 180.0)
 
 
 @pytest.mark.skipif(os.environ.get("CUOPT_B200_LONG_TESTS") != "1",
-                    reason="5-10 minutes of one B200: run with CUOPT_B200_LONG_TESTS=1 (last run: profiles/r2/)")
+                    reason="several minutes of one GPU: run with CUOPT_B200_LONG_TESTS=1")
 def test_headline_lp_converges_to_the_planted_optimum():
     """configs[3] at tolerance 1e-6 (the "time-to-1e-6-gap" solve of bench.py): Optimal, both objectives within 1e-5 of the
-    planted optimum.  The 1e-6 accuracy on the objectives themselves needs tolerance ~1e-7 here, i.e. > 550 000 iterations /
-    10 minutes on one B200: measured once (profiles/r2/time_to_tolerance_c4_1e-7.txt: 4.7e-7 primal, 2.2e-7 dual after
-    551 800 iterations), not part of the suite."""
+    planted optimum.  The 1e-6 accuracy on the objectives themselves needs tolerance ~1e-7 here, i.e. several hundred
+    thousand iterations, not part of the suite."""
     solve_to_planted_optimum(10_000_000, 1e-6, 1e-5, 600.0)

@@ -2,8 +2,7 @@
 (cuopt_b200/csrc/trust_region.cuh), against the oracle restatement that is pinned to the reference's tests:
   * the reference's test_very_low_tolerance (test_lp_solver.py:101-121),
   * the iterates across the first trust-region restarts against the oracle,
-  * the objectives of the golden instances (the oracle's are pinned to the reference's dual simplex).
-First GPU run: round 2 (gpurun_out r2a); the environment gate of round 1 is gone."""
+  * the objectives of the golden instances (the oracle's are pinned to the reference's dual simplex)."""
 import numpy as np
 import pytest
 
@@ -17,11 +16,8 @@ pytestmark = pytest.mark.gpu
 # 6 x 64 steps crossing trust-region restarts (sort + prefix sums + bisection feed the restart decision), iterates compared
 # with the sequential oracle at every checkpoint.  PDHG with adaptive steps is a discontinuous map (accept / reject, restart
 # candidate): two summation orders of the same algorithm agree to rounding for a while and then part ways while converging to
-# the same solution.  Measured on the B200 (worst vector, checkpoints 1..6):
-#   round-1 SpMV core (row sums bit-identical to the oracle's):  ... 1.6e-7 at checkpoint 6
-#   block-interleaved core (rows that span lanes: carry + part): 8.8e-9, 6.2e-8, 1.1e-4, 1.5e-4, 1.9e-2, 2.8e-2
-# with the SAME number of trust-region restarts (1, 2, 2, 3, 3, 3) at every checkpoint.  Asserted: rounding-level agreement
-# over the first 128 steps (two restarts), equal restart counts throughout, and no blow-up afterwards; the end result of
+# the same solution: the block-interleaved core (rows that span lanes: carry + part) adds in another order than the oracle,
+# and the grids follow the device's SM count.  Asserted: rounding-level agreement over the first 128 steps (two restarts), equal restart counts throughout, and no blow-up afterwards; the end result of
 # the preset is pinned by the other tests of this file.
 CHECKPOINT_BOUNDS = [1e-6, 1e-6, 1e-1, 1e-1, 1e-1, 1e-1]
 

@@ -7,7 +7,7 @@ Sources of truth (all committed under tests/golden/, produced by scripts/gen_gol
 import numpy as np
 import pytest
 
-from conftest import mps_path, problem_arrays
+from conftest import load_golden, mps_path, problem_arrays
 from cuopt_b200 import capi
 from oracle import pdlp_oracle as po
 
@@ -176,9 +176,7 @@ def c_api_infeasible_lp():
 def test_infeasibility_detection_on_the_reference_c_api_infeasible_lp(strict):
     off, idx, val, c, l, u, lc, uc = c_api_infeasible_lp()
     # the reference's own verdict on it (its test expects CUOPT_TERIMINATION_STATUS_INFEASIBLE from the dual simplex)
-    from oracle import ref_cpu
-    if ref_cpu.available():
-        assert ref_cpu.dual_simplex(off, idx, val, lc, uc, c, l, u)["status"] == "INFEASIBLE"
+    assert reference_verdict("c_api_infeasible_lp", off, idx, val, c, l, u, lc, uc) == "INFEASIBLE"
     o = po.Oracle(off, idx, val, c, l, u, lc, uc, tol=1e-4, detect_infeasibility=True, strict_infeasibility=strict,
                   iteration_limit=100000)
     assert o.run(-1)
@@ -189,14 +187,24 @@ def test_infeasibility_detection_on_the_reference_c_api_infeasible_lp(strict):
     assert o.stats().termination_status == 4
 
 
-def test_infeasibility_detection_flags_an_unbounded_lp():
+def unbounded_lp():
     # min -x  s.t.  x - y = 0,  x, y >= 0: the ray (1, 1) improves forever
-    inf = np.inf
     off, idx, val = np.array([0, 2], np.int32), np.array([0, 1], np.int32), np.array([1.0, -1.0])
-    args = (off, idx, val, np.array([-1.0, 0.0]), np.zeros(2), np.full(2, inf), np.zeros(1), np.zeros(1))
+    return off, idx, val, np.array([-1.0, 0.0]), np.zeros(2), np.full(2, np.inf), np.zeros(1), np.zeros(1)
+
+
+def reference_verdict(name, off, idx, val, c, l, u, lc, uc):
+    """The reference CPU dual simplex's status: run live where oracle/_ref is built, else as stored by
+    scripts/gen_golden_writer.py."""
     from oracle import ref_cpu
     if ref_cpu.available():
-        assert ref_cpu.dual_simplex(off, idx, val, args[6], args[7], args[3], args[4], args[5])["status"] == "UNBOUNDED"
+        return ref_cpu.dual_simplex(off, idx, val, lc, uc, c, l, u)["status"]
+    return load_golden("writer_golden.json")["verdicts"][name]
+
+
+def test_infeasibility_detection_flags_an_unbounded_lp():
+    args = unbounded_lp()
+    assert reference_verdict("unbounded_lp", *args) == "UNBOUNDED"
     o = po.Oracle(*args, tol=1e-4, detect_infeasibility=True, strict_infeasibility=True, iteration_limit=100000)
     assert o.run(-1)
     assert o.stats().termination_status == 3   # DualInfeasible == CUOPT_TERIMINATION_STATUS_UNBOUNDED

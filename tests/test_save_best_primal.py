@@ -47,6 +47,6 @@ def test_gpu_matches_the_oracle(rel, limit):
     st = sol.stats()
     assert st.number_of_steps_taken == want.number_of_steps_taken
     # same recorded iterate (equal step counts); values to the drift of a 100-300 step trajectory on these degenerate
-    # relaxations (measured on the B200: 5e-6 on 50v-10, < 1e-6 on the other two)
+    # relaxations
     assert st.l2_primal_residual == pytest.approx(want.l2_primal_residual, rel=1e-4, abs=1e-9)
     assert st.primal_objective == pytest.approx(want.primal_objective, rel=1e-4, abs=1e-9)
