@@ -19,7 +19,7 @@
 // fixed grid, so results are bit-reproducible run to run.  For large LPs K2 / K3 are split by column blocks ("gather
 // blocking", further down) with the row epilogue fused into the LAST block's pass; the sharded multi-GPU attempt and its
 // NVLink peer transport follow the single-GPU kernels; the evaluation / infeasibility kernels are element-wise over
-// products formed by k_spmv.  DESIGN.md §5 describes these choices and their measurements.
+// products formed by k_spmv_pair (both iterates in one stream of the unscaled matrix, over its column blocks when blocked).  DESIGN.md §5 describes these choices and their measurements.
 #pragma once
 
 #include "device_utils.cuh"
@@ -970,6 +970,26 @@ __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_spmv(bicsr_vi
   auto pre_op = [&](int) { return payload_t{}; };
   auto row_op = [&](int i, double s, const payload_t&) { out[i] = s; };
   spmv_bicsr_rows<payload_t>(A, x, rows[threadIdx.x >> 5], pre_op, row_op, make_l2_policies(g_l2_hints).keep);
+}
+
+// Products of the termination evaluation, current and average iterate in ONE stream of the (unscaled) matrix:
+//   out_u = M u, out_v = M v  (first),   out_u += M u, out_v += M v  (otherwise).
+// A gather-blocked matrix runs one launch per column block, in block order (first = block 0): the sums of a row come out in
+// the order of k_block_pass.  An unblocked matrix is one first pass, whose sums are exactly k_spmv's.
+__global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_spmv_pair(bicsr_view_t M,
+                                                                             const double* __restrict__ u,
+                                                                             const double* __restrict__ v,
+                                                                             double* __restrict__ out_u,
+                                                                             double* __restrict__ out_v,
+                                                                             int first)
+{
+  __shared__ double rows[2][BICSR_WARPS][BICSR_SLOTS];
+  auto row_op = [&](int r, double su, double sv) {
+    out_u[r] = first ? su : out_u[r] + su;
+    out_v[r] = first ? sv : out_v[r] + sv;
+  };
+  const int w = threadIdx.x >> 5;
+  spmv_bicsr_rows_pair(M, u, v, rows[0][w], rows[1][w], row_op, make_l2_policies(g_l2_hints).keep);
 }
 
 // =============================================================================================

@@ -428,6 +428,7 @@ struct pdlp_solver_t::impl_t {
   struct gather_blocks_t {
     int B = 1, width = 0;
     std::vector<csr_dev_t> blk;
+    std::vector<csr_dev_t> unscaled;  // single GPU: the same blocks with the unscaled values (termination evaluation)
     std::vector<int> grid;  // per block, for the schedule (wide or not) its pass uses
     bool on() const { return B > 1; }
   };
@@ -892,8 +893,8 @@ struct pdlp_solver_t::impl_t {
     if (sharded() && dist_mode == DIST_GATHER) {
       build_gather_transport();  // packed A_g, rows J_g of the global A^T; the hot loop never multiplies by A_g^T
     } else {
-      build_gather_blocks(As, blkA, t_m);
-      build_gather_blocks(ATs, blkAT, t_n);
+      build_gather_blocks(As, blkA, t_m, 0, sharded() ? nullptr : &A);
+      build_gather_blocks(ATs, blkAT, t_n, 0, sharded() ? nullptr : &AT);
     }
     trace.mark("gather blocks");
     n_part_dy2 = k2_grid();  // CTAs of the kernel that runs the dual row epilogue
@@ -1172,7 +1173,9 @@ struct pdlp_solver_t::impl_t {
   // ------------------------------------------------------------------------------ PDHG batches
   // Cuts the scaled matrix M into column blocks (device, stable) when the vector it gathers from exceeds the block size.
   // forced_width > 0 (gather transport): exactly two blocks, cut at that column, whatever the size of the gathered vector
-  void build_gather_blocks(const csr_dev_t& M, gather_blocks_t& g, dvec<double>& t, int forced_width = 0)
+  // unscaled_src: the unscaled matrix M is a scaled copy of; its values are split into g.unscaled along the same cut
+  void build_gather_blocks(const csr_dev_t& M, gather_blocks_t& g, dvec<double>& t, int forced_width = 0,
+                           const csr_dev_t* unscaled_src = nullptr)
   {
     g = gather_blocks_t{};
     const size_t bytes = (size_t)M.cols * sizeof(double);
@@ -1216,6 +1219,27 @@ struct pdlp_solver_t::impl_t {
       sync();
       build_bicsr(g.blk[b], hoff, stream, sms);
       g.grid[b] = spmv_grid(g.blk[b]);
+    }
+    if (unscaled_src) {  // the cut depends on the structure only, which M shares with unscaled_src
+      g.unscaled.resize(B);
+      for (int b = 0; b < B; ++b) {
+        csr_dev_t& U = g.unscaled[b];
+        U.rows = M.rows; U.cols = M.cols; U.nnz = nnz_b[b];
+        U.structure = &g.blk[b];
+        U.val.resize((size_t)nnz_b[b]);
+        vals[b] = U.val.data();
+      }
+      // rewrites the blocks' column indices with the same values
+      csr_split_columns_fill(M.rows, M.off_ptr(), M.idx_ptr(), unscaled_src->val.data(), g.width, B, offs.data(), idxs.data(),
+                             vals.data(), stream);
+      for (csr_dev_t& U : g.unscaled) {
+        fill_bicsr_values(U, stream, sms);
+        // the plain values serve the long-row blocks only (bicsr_view_t::cval): without such rows only the BICSR values stay
+        if (U.bi_structure().n_std == U.bi_structure().n_blk) {
+          sync();
+          U.val = dvec<double>{};
+        }
+      }
     }
     t.resize((size_t)M.rows);
     t.zero(stream);
@@ -1307,6 +1331,18 @@ struct pdlp_solver_t::impl_t {
   void launch_spmv(const csr_dev_t& M, const double* v, double* out)
   {
     k_spmv<<<spmv_grid(M), BICSR_THREADS, 0, stream>>>(M.view(), v, out);
+  }
+  // out_u = M u, out_v = M v for the unscaled M, over the unscaled column blocks g holds of it (else in one pass); returns
+  // the number of launches
+  int launch_spmv_pair(const csr_dev_t& M, const gather_blocks_t& g, const double* u, const double* v, double* out_u,
+                       double* out_v)
+  {
+    const int count = g.unscaled.empty() ? 1 : (int)g.unscaled.size();
+    for (int b = 0; b < count; ++b) {
+      const csr_dev_t& Mb = g.unscaled.empty() ? M : g.unscaled[b];
+      k_spmv_pair<<<spmv_grid(Mb), BICSR_THREADS, 0, stream>>>(Mb.view(), u, v, out_u, out_v, b == 0);
+    }
+    return count;
   }
 
   // scheme (ii): this rank updates only its slice of the primal side (kernel comments in pdlp_kernels.cuh)
@@ -1457,14 +1493,19 @@ struct pdlp_solver_t::impl_t {
     if (steps <= 0) return;
     nvtx_range_t nvtx_scope("take_step batch (PDHG attempts up to the next major iteration)");
     CUOPT_CUDA_TRY(cudaEventRecord(ev_a, stream));
+    k_begin_batch<<<1, 1, 0, stream>>>(d_ctl.data(), steps);  // first: the block passes below run only in an active batch
     if (need_aty) {  // pdhg.cu:183-202
       const int cur = h_ctl->parity;
-      launch_spmv(ATs, ybuf[cur].data(), atybuf[cur].data());
+      if (blkAT.on() && !sharded()) {  // summed over the column blocks exactly as K3 sums A^T y'
+        launch_block_passes(blkAT, blkAT.B, ybuf[cur].data(), ybuf[cur].data(), 0, atybuf[cur].data(), nullptr, 0);
+        launches += blkAT.B;
+      } else {
+        launch_spmv(ATs, ybuf[cur].data(), atybuf[cur].data());
+        ++launches;
+      }
       if (sharded()) dist->allreduce(atybuf[cur].data(), n, false, stream);
-      ++launches;
       need_aty = false;
     }
-    k_begin_batch<<<1, 1, 0, stream>>>(d_ctl.data(), steps);
     const int target = h_ctl->accepted + steps;
     int todo         = steps;
     while (true) {
@@ -1529,14 +1570,12 @@ struct pdlp_solver_t::impl_t {
                                                              x_avg.data(), Dc.data());
     k_average_and_unscale<<<grid_m, EW_THREADS, 0, stream>>>(d_ctl.data(), mode, m, ybuf[cur].data(), sum_y.data(),
                                                              y_avg.data(), Dr.data());
-    launch_spmv(A, xbuf[cur].data(), eval_m.data());
-    launch_spmv(A, x_avg.data(), eval_m.data() + m);
+    launches += launch_spmv_pair(A, blkA, xbuf[cur].data(), x_avg.data(), eval_m.data(), eval_m.data() + m);
     k_eval_rows_from_ax<<<grid_m, EW_THREADS, 0, stream>>>(m, eval_m.data(), eval_m.data() + m, ybuf[cur].data(),
                                                            y_avg.data(), lc.data(), uc.data(), part_rows.data(),
                                                            st.relative_primal_tolerance,
                                                            st.per_constraint_residual ? part_max.data() : nullptr);
     const int n_rows_parts = grid_m;
-    launches += 2;
     {
       // A^T y for both iterates, then the column math element-wise.  Row-sharded: the six row sums and both products
       // are partial and are combined over the ranks first.
@@ -1549,8 +1588,7 @@ struct pdlp_solver_t::impl_t {
         rows_src   = d_scalar.data();
         rows_count = 1;
       }
-      launch_spmv(AT, ybuf[cur].data(), aty2);
-      launch_spmv(AT, y_avg.data(), aty2 + n);
+      launches += launch_spmv_pair(AT, blkAT, ybuf[cur].data(), y_avg.data(), aty2, aty2 + n);
       if (sharded()) dist->allreduce(aty2, 2 * (size_t)n, false, stream);
       double* max_cols       = nullptr;
       const double* max_rows = nullptr;
@@ -1570,7 +1608,7 @@ struct pdlp_solver_t::impl_t {
                                                               c.data(), l.data(), u.data(), rc_cur.data(), rc_avg.data(),
                                                               part_cols.data(), rows_src, rows_count, eval_consts(),
                                                               d_eval.data(), max_cols, max_rows, max_rows_count);
-      launches += 3;
+      launches += 1;
       if (st.detect_infeasibility) {  // single GPU only (checked in build)
         double* rows_parts = part_infeas.data();
         double* cols_parts = part_infeas.data() + 6 * (size_t)grid_m;
@@ -2034,6 +2072,9 @@ double pdlp_solver_t::scalar(const std::string& name)
   if (name == "last_restart_kkt") return s.last_restart_kkt;
   if (name == "last_candidate_kkt") return s.last_candidate_kkt;
   if (name == "n_restarts") return s.sol.stats.n_restarts;
+  if (name == "last_restart_was_average") return s.last_restart_was_average ? 1.0 : 0.0;
+  if (name == "eval_blocks") return (double)std::max<size_t>(1, s.blkA.unscaled.size());  // passes of the evaluation's A x
+  if (name == "eval_blocks_t") return (double)std::max<size_t>(1, s.blkAT.unscaled.size());
   if (name == "valid") return k.valid;
   return std::nan("");
 }

@@ -54,6 +54,38 @@ struct bicsr_view_t {
   const double* cval;
 };
 
+// Steps 3-4 of the core for one gathered vector: bit k of `ends` = entry k of this lane closes a row; the sum of every row
+// that ends in this lane's chunk goes to rsw[slot of its last entry].
+__device__ __forceinline__ void bicsr_block_row_sums(const double (&a)[BICSR_CH], const double (&g)[BICSR_CH], unsigned ends,
+                                                     int lane, double* rsw)
+{
+  constexpr unsigned FULL = 0xffffffffu;
+  // chunk sums, left to right, branch-free; the FIRST row end of the chunk still lacks what earlier lanes hold of that row
+  double s = 0.0, head = 0.0;
+  const int kf = ends ? __ffs(ends) - 1 : -1;
+#pragma unroll
+  for (int k = 0; k < BICSR_CH; ++k) {
+    s = __dadd_rn(s, __dmul_rn(a[k], g[k]));  // product, then sum: no FMA contraction (the CPU oracle has none either)
+    const bool e = (ends >> k) & 1u;
+    if (e && k != kf) rsw[k * 32 + lane] = s;
+    head = (k == kf) ? s : head;
+    s    = e ? 0.0 : s;
+  }
+  // carry = what the lanes before this one hold of the row that is open at this lane's first entry.  A lane without any
+  // row end passes its whole chunk on; runs of such lanes need one more shuffle round each.
+  double tail  = s;
+  double carry = __shfl_up_sync(FULL, tail, 1);
+  if (lane == 0) carry = 0.0;
+  unsigned pending = __ballot_sync(FULL, kf < 0);
+  while (pending) {
+    if (kf < 0) tail = carry + s;
+    carry = __shfl_up_sync(FULL, tail, 1);
+    if (lane == 0) carry = 0.0;
+    pending &= pending << 1;
+  }
+  if (kf >= 0) rsw[kf * 32 + lane] = carry + head;
+}
+
 // Walks this warp's blocks.
 //   pre_op(row)            -> payload P (vector operands of the row epilogue; issued before the matrix loads for the first
 //                             32 rows of a block, so their latency hides behind the gathers)
@@ -71,7 +103,6 @@ __device__ __forceinline__ void spmv_bicsr_rows(const bicsr_view_t& A,
                                                 RowOp& row_op,
                                                 unsigned long long gather_policy)
 {
-  constexpr unsigned FULL = 0xffffffffu;
   const int lane          = threadIdx.x & 31;
   const int gwarp         = blockIdx.x * BICSR_WARPS + (threadIdx.x >> 5);
   const int nwarps        = gridDim.x * BICSR_WARPS;
@@ -109,30 +140,7 @@ __device__ __forceinline__ void spmv_bicsr_rows(const bicsr_view_t& A,
 #pragma unroll
       for (int k = 0; k < BICSR_CH; ++k) c[k] = ld_stream(A.idx + (size_t)(b + nwarps) * BICSR_SLOTS + k * 32 + lane);
     }
-    // chunk sums, left to right, branch-free; the FIRST row end of the chunk still lacks what earlier lanes hold of that row
-    double s = 0.0, head = 0.0;
-    const int kf = ends ? __ffs(ends) - 1 : -1;
-#pragma unroll
-    for (int k = 0; k < BICSR_CH; ++k) {
-      s = __dadd_rn(s, __dmul_rn(a[k], g[k]));  // product, then sum: no FMA contraction (the CPU oracle has none either)
-      const bool e = (ends >> k) & 1u;
-      if (e && k != kf) rsw[k * 32 + lane] = s;
-      head = (k == kf) ? s : head;
-      s    = e ? 0.0 : s;
-    }
-    // carry = what the lanes before this one hold of the row that is open at this lane's first entry.  A lane without any
-    // row end passes its whole chunk on; runs of such lanes need one more shuffle round each.
-    double tail  = s;
-    double carry = __shfl_up_sync(FULL, tail, 1);
-    if (lane == 0) carry = 0.0;
-    unsigned pending = __ballot_sync(FULL, kf < 0);
-    while (pending) {
-      if (kf < 0) tail = carry + s;
-      carry = __shfl_up_sync(FULL, tail, 1);
-      if (lane == 0) carry = 0.0;
-      pending &= pending << 1;
-    }
-    if (kf >= 0) rsw[kf * 32 + lane] = carry + head;
+    bicsr_block_row_sums(a, g, ends, lane, rsw);
     __syncwarp();
 #pragma unroll
     for (int q = 0; q < NPRE; ++q) {
@@ -164,6 +172,65 @@ __device__ __forceinline__ void spmv_bicsr_rows(const bicsr_view_t& A,
       if constexpr (INIT) acc = pl.init + acc;
       row_op(row, acc, pl);
     }
+  }
+}
+
+// Two vectors through ONE stream of the matrix: row_op(row, (M u)_row, (M v)_row) exactly once per row, by the same lane as
+// in spmv_bicsr_rows.  Each sum is formed exactly as spmv_bicsr_rows forms it.  rsw_u / rsw_v: BICSR_SLOTS doubles each.
+// No payload is fetched ahead and the next block's indices are not prefetched: the 16 gathers of a block already keep the
+// warp's loads in flight, and the registers go to the second set of gathered values.
+template <typename RowOp>
+__device__ __forceinline__ void spmv_bicsr_rows_pair(const bicsr_view_t& A,
+                                                     const double* __restrict__ u,
+                                                     const double* __restrict__ v,
+                                                     double* rsw_u,
+                                                     double* rsw_v,
+                                                     RowOp& row_op,
+                                                     unsigned long long gather_policy)
+{
+  const int lane   = threadIdx.x & 31;
+  const int gwarp  = blockIdx.x * BICSR_WARPS + (threadIdx.x >> 5);
+  const int nwarps = gridDim.x * BICSR_WARPS;
+  for (int b = gwarp; b < A.n_std; b += nwarps) {
+    const int2 d      = __ldg(A.desc + b);
+    const size_t base = (size_t)b * BICSR_SLOTS + lane;
+    int c[BICSR_CH];
+    double a[BICSR_CH], gu[BICSR_CH], gv[BICSR_CH];
+#pragma unroll
+    for (int k = 0; k < BICSR_CH; ++k) c[k] = ld_stream(A.idx + base + k * 32);
+#pragma unroll
+    for (int k = 0; k < BICSR_CH; ++k) a[k] = ld_stream(A.val + base + k * 32);
+#pragma unroll
+    for (int k = 0; k < BICSR_CH; ++k) {
+      const int col = c[k] & 0x7fffffff;
+      gu[k]         = col != BICSR_PAD ? ld_l2(u + col, gather_policy) : 0.0;
+      gv[k]         = col != BICSR_PAD ? ld_l2(v + col, gather_policy) : 0.0;
+    }
+    unsigned ends = 0;
+#pragma unroll
+    for (int k = 0; k < BICSR_CH; ++k) ends |= (unsigned)(c[k] < 0) << k;
+    bicsr_block_row_sums(a, gu, ends, lane, rsw_u);
+    bicsr_block_row_sums(a, gv, ends, lane, rsw_v);
+    __syncwarp();
+    for (int r = d.x + lane; r < d.y; r += 32) {
+      const unsigned short s = __ldg(A.row_slot + r);
+      row_op(r, s != BICSR_EMPTY ? rsw_u[s] : 0.0, s != BICSR_EMPTY ? rsw_v[s] : 0.0);
+    }
+    __syncwarp();
+  }
+  for (int b = A.n_std + gwarp; b < A.n_blk; b += nwarps) {
+    const int row = __ldg(A.desc + b).x;
+    const int lo = __ldg(A.off + row), hi = __ldg(A.off + row + 1);
+    double acc_u = 0.0, acc_v = 0.0;
+    for (int e = lo + lane; e < hi; e += 32) {
+      const double a = ld_stream(A.cval + e);
+      const int col  = ld_stream(A.cidx + e);
+      acc_u += a * ld_l2(u + col, gather_policy);
+      acc_v += a * ld_l2(v + col, gather_policy);
+    }
+    acc_u = warp_sum(acc_u);
+    acc_v = warp_sum(acc_v);
+    if (lane == 0) row_op(row, acc_u, acc_v);
   }
 }
 
