@@ -148,7 +148,7 @@ __device__ __forceinline__ void pdhg_step_rule(pdhg_ctl_t* ctl, double interacti
 // ---- multi-GPU peer transport primitives (used by the column-sliced attempt further down) ----
 constexpr int DIST_MAX_PEERS        = 8;
 constexpr int DIST_FLAG_XBAR        = 0 * DIST_MAX_PEERS;  // flags[slot + g]: rank g's contribution has landed
-constexpr int DIST_FLAG_PARTIAL     = 1 * DIST_MAX_PEERS;  // partial A_g^T y' (p2p transport) / first half of y' (gather transport)
+constexpr int DIST_FLAG_Y           = 1 * DIST_MAX_PEERS;  // gather transport: first half of rank g's y' entries
 constexpr int DIST_FLAG_SCALARS     = 2 * DIST_MAX_PEERS;
 constexpr int DIST_FLAG_XBAR_B      = 3 * DIST_MAX_PEERS;  // gather transport: second half of rank g's xbar entries
 constexpr int DIST_FLAG_Y_B         = 4 * DIST_MAX_PEERS;  // gather transport: second half of rank g's y' entries
@@ -315,7 +315,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_dual_st
   spmv_bicsr_rows<payload_t, INIT, NPRE>(A, xbar, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
   const double tot = block_reduce(dy2, red);
   if (threadIdx.x == 0) part_dy2[blockIdx.x] = tot;
-  if constexpr (BCAST) peer_signal_grid_done(&ctl->ticket[2], flags, world, DIST_FLAG_PARTIAL + rank, epoch, DIST_FLAG_Y_B + rank);
+  if constexpr (BCAST) peer_signal_grid_done(&ctl->ticket[2], flags, world, DIST_FLAG_Y + rank, epoch, DIST_FLAG_Y_B + rank);
 }
 
 // =============================================================================================
@@ -379,7 +379,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_transpo
 // A^T y' on its slice is a complete row sum over the all-gathered y' (yfull: every rank's K2 stores its rows there) —
 // no partial products, no reduce-scatter, and per rank exactly 1/G of the single-GPU K3.  Row j is LOCAL to the slice
 // (the x / A^T y pointers are offset by the slice start).  Tail: {interaction, ||dx||^2 of the slice, ||dy||^2 of this
-// rank's rows} go to the scalar table of every rank (as in k_interaction_slice); k_step_rule_gather follows.
+// rank's rows} go to the scalar table of every rank; k_step_rule_gather follows.
 template <bool INIT, int NPRE>
 __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_transpose_step_slice(pdhg_ctl_t* __restrict__ ctl,
                                                                                         bicsr_view_t AT,
@@ -627,9 +627,8 @@ __global__ void __launch_bounds__(EW_THREADS) k_remap_indices(int nnz, const int
 }
 
 // ---------------------------------------------------------------------------------------------
-// Row-sharded (multi-GPU) variants of K3.  Each rank owns a block of rows of A; A_g^T y'_g is a PARTIAL
-// A^T y' that is summed over ranks (NCCL all-reduce on the solver stream) between K3a and K3b.  The extra slot
-// buf[n] carries this rank's ||dy||^2 through the same collective.
+// Row-sharded (multi-GPU) K3 of the NCCL transport.  Each rank owns a block of rows of A; A_g^T y'_g is a PARTIAL
+// A^T y' over all n columns that the reduce-scatter sums over ranks into the slice owners (k_interaction_slice).
 // ---------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_transpose_partial(const pdhg_ctl_t* __restrict__ ctl,
                                                                                      bicsr_view_t AT,
@@ -646,13 +645,11 @@ __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_transpose_par
   spmv_bicsr_rows<payload_t>(AT, yn, rows[threadIdx.x >> 5], pre_op, row_op, make_l2_policies(g_l2_hints).keep);
 }
 // buf[slot] = sum of `count` per-CTA partials (one CTA, fixed order)
-__global__ void __launch_bounds__(EW_THREADS) k_sum_partials(const pdhg_ctl_t* __restrict__ ctl,
-                                                             const double* __restrict__ parts,
+__global__ void __launch_bounds__(EW_THREADS) k_sum_partials(const double* __restrict__ parts,
                                                              int count,
                                                              int n_quantities,
                                                              double* __restrict__ out)
 {
-  if (ctl && !ctl->active) return;
   __shared__ double red[32];
   for (int q = 0; q < n_quantities; ++q) {
     double s = 0.0;
@@ -661,55 +658,29 @@ __global__ void __launch_bounds__(EW_THREADS) k_sum_partials(const pdhg_ctl_t* _
     if (threadIdx.x == 0) out[q] = s;
   }
 }
-// K3b: after the all-reduce buf = A^T y' (global) and buf[n] = ||dy||^2 (global)
-__global__ void __launch_bounds__(EW_THREADS) k_interaction_step(pdhg_ctl_t* __restrict__ ctl,
-                                                                 int n,
-                                                                 const double* __restrict__ buf,
-                                                                 const double* __restrict__ xbuf0,
-                                                                 const double* __restrict__ xbuf1,
-                                                                 double* __restrict__ aty0,
-                                                                 double* __restrict__ aty1,
-                                                                 double* __restrict__ parts)
-{
-  if (!ctl->active) return;
-  __shared__ double red[32];
-  const int cur     = ctl->parity;
-  const double* x   = cur ? xbuf1 : xbuf0;
-  const double* xn  = cur ? xbuf0 : xbuf1;
-  const double* aty = cur ? aty1 : aty0;
-  double* atyn      = cur ? aty0 : aty1;
-  double acc[2]     = {0.0, 0.0};
-  const int stride  = gridDim.x * blockDim.x;
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
-    const double s = buf[j];
-    atyn[j]        = s;
-    const double d = xn[j] - x[j];
-    acc[0] += d * (s - aty[j]);
-    acc[1] += d * d;
-  }
-  if (!publish_and_elect<2>(acc, parts, &ctl->ticket[0], red)) return;
-  const double interaction = gather_partials(parts, gridDim.x, red);
-  const double dx2         = gather_partials(parts + gridDim.x, gridDim.x, red);
-  if (threadIdx.x != 0) return;
-  pdhg_step_rule(ctl, interaction, dx2, __ldcg(buf + n));
-}
 
 // ---------------------------------------------------------------------------------------------
 // Column-sliced multi-GPU attempt (SURVEY §8e scheme (ii)): rank g owns rows R_g of A AND the slice
-// J_g = [g*nslice, (g+1)*nslice) of every primal vector.  Per attempt
-//   K1s   primal step on J_g; xbar slice -> every rank           (all-gather)
-//   K2    dual step on R_g (needs the full xbar)
-//   K3p   partial A_g^T y'_g over all n columns -> slice owners  (reduce-scatter)
-//   K3s   owner sums the G partials of its slice in rank order, interaction / movement partial sums
+// J_g = [g*nslice, (g+1)*nslice) of every primal vector.  Two transports.
+// gather (default): rank g also owns the rows J_g of the global A^T, so both products take all-gathered inputs and
+// there are no partial products.  The producing kernels store what each rank reads into its packed buffers
+// themselves (NVLink peer stores that overlap the work; flags replace the collectives, no NCCL in the loop):
+//   K1s   primal step on J_g; xbar entries -> the ranks that read them   (k_primal_step_bcast)
+//   K2    dual step on R_g over the packed xbar; y' entries -> the ranks that read them   (k_dual_step<..., true>)
+//   K3s   A^T y' on J_g over the all-gathered y', interaction / movement partial sums   (k_transpose_step_slice)
 //   rule  three scalars from every rank, summed in rank order -> identical accept/reject everywhere
-// Two transports: NCCL collectives between the kernels, or NVLink peer stores issued by the producing kernels
-// themselves (the transfer overlaps the SpMV row by row; flags replace the collectives, no NCCL in the loop).
 // Flags are monotone epochs (= attempt number), written with st.release.sys by the last CTA of the producer
 // after every CTA fenced its stores system-wide; consumers poll with ld.acquire.sys and read the payload
 // with ld.global.cg (L2 is the coherence point for peer writes).
+// nccl (selectable, and the fallback when the GPUs cannot map each other's memory): NCCL collectives between the kernels
+//   K1s   primal step on J_g; xbar slice -> every rank           (all-gather)
+//   K2    dual step on R_g (needs the full xbar)
+//   K3p   partial A_g^T y'_g over all n columns -> slice owners  (reduce-scatter)
+//   K3s   interaction / movement partial sums on J_g             (k_interaction_slice)
+//   rule  three scalars from every rank, summed over the ranks   (all-reduce)
 // ---------------------------------------------------------------------------------------------
-// K1s with the all-gather fused in: pointers are already offset to this rank's slice; xbar_peers.p[r] = rank r's
-// xbar + j0.
+// K1s with the xbar exchange fused in: pointers are already offset to this rank's slice; send[r * send_stride + j] = slot
+// of x_j in rank r's packed xbar (xbar_peers.p[r]), -1 if rank r never reads it.
 __global__ void __launch_bounds__(EW_THREADS) k_primal_step_bcast(pdhg_ctl_t* __restrict__ ctl,
                                                                   int nloc,
                                                                   double* __restrict__ xbuf0,
@@ -724,8 +695,8 @@ __global__ void __launch_bounds__(EW_THREADS) k_primal_step_bcast(pdhg_ctl_t* __
                                                                   peer_flags_t flags,
                                                                   int world,
                                                                   int rank,
-                                                                  const int* __restrict__ send = nullptr,
-                                                                  int send_stride = 0)
+                                                                  const int* __restrict__ send,
+                                                                  int send_stride)
 {
   if (!ctl->active) return;
   const unsigned long long epoch = (unsigned long long)ctl->attempts + 1ull;
@@ -745,61 +716,22 @@ __global__ void __launch_bounds__(EW_THREADS) k_primal_step_bcast(pdhg_ctl_t* __
     next                  = fmax(fmin(next, ld_stream(u + j)), ld_stream(l + j));
     xn[j]                 = next;
     const double xb       = next - xj + next;
-    if (send) {  // gather transport: packed xbar, send[r * send_stride + j] = slot in rank r's buffer, -1 if r never reads x_j
 #pragma unroll
-      for (int r = 0; r < DIST_MAX_PEERS; ++r)
-        if (r < world) {
-          const int d = __ldg(send + (size_t)r * send_stride + j);
-          if (d >= 0) xbar_peers.p[r][d] = xb;
-        }
-    } else {
-#pragma unroll
-      for (int r = 0; r < DIST_MAX_PEERS; ++r)
-        if (r < world) xbar_peers.p[r][j] = xb;
-    }
+    for (int r = 0; r < DIST_MAX_PEERS; ++r)
+      if (r < world) {
+        const int d = __ldg(send + (size_t)r * send_stride + j);
+        if (d >= 0) xbar_peers.p[r][d] = xb;
+      }
   }
-  peer_signal_grid_done(&ctl->ticket[1], flags, world, DIST_FLAG_XBAR + rank, epoch, send ? DIST_FLAG_XBAR_B + rank : -1);
+  peer_signal_grid_done(&ctl->ticket[1], flags, world, DIST_FLAG_XBAR + rank, epoch, DIST_FLAG_XBAR_B + rank);
 }
 
-// K3p with the reduce-scatter fused in: column j's partial goes straight to its owner's staging row of this rank;
-// stage_peers.p[h] = rank h's stage + rank * nslice.
-__global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_transpose_partial_scatter(pdhg_ctl_t* __restrict__ ctl,
-                                                                                             bicsr_view_t AT,
-                                                                                             const double* __restrict__ ybuf0,
-                                                                                             const double* __restrict__ ybuf1,
-                                                                                             peer_ptrs_t stage_peers,
-                                                                                             int nslice,
-                                                                                             peer_flags_t flags,
-                                                                                             int world,
-                                                                                             int rank)
-{
-  if (!ctl->active) return;
-  __shared__ double rows[BICSR_WARPS][BICSR_SLOTS];
-  const unsigned long long epoch = (unsigned long long)ctl->attempts + 1ull;
-  const double* yn               = ctl->parity ? ybuf0 : ybuf1;
-  struct payload_t {};
-  auto pre_op = [&](int) { return payload_t{}; };
-  auto row_op = [&](int j, double s, const payload_t&) {
-    const int h  = j / nslice;
-    double* base = stage_peers.p[0];
-#pragma unroll
-    for (int r = 1; r < DIST_MAX_PEERS; ++r)
-      if (h == r) base = stage_peers.p[r];
-    base[j - h * nslice] = s;
-  };
-  spmv_bicsr_rows<payload_t>(AT, yn, rows[threadIdx.x >> 5], pre_op, row_op, make_l2_policies(g_l2_hints).keep);
-  peer_signal_grid_done(&ctl->ticket[2], flags, world, DIST_FLAG_PARTIAL + rank, epoch);
-}
-
-// K3s: A^T y' on this rank's slice = sum over the n_src staged partials (rank order), then the slice's share of
-// the interaction and ||dx||^2; the last CTA hands {interaction, ||dx||^2, ||dy||^2 of this rank's rows} to
-// every rank in scal_peers (p[r] = rank r's scalar table + 4 * rank) and raises the scalar flag.
-// NCCL transport: n_src = 1 (src = reduce-scatter output), world_out = 1, flags.p[0] = nullptr.
+// K3s (NCCL transport): A^T y' on this rank's slice = the reduce-scatter output src, then the slice's share of the
+// interaction and ||dx||^2; the last CTA writes {interaction, ||dx||^2, ||dy||^2 of this rank's rows} to scal[0..3),
+// which the all-reduce sums over the ranks before k_step_rule_gather.
 __global__ void __launch_bounds__(EW_THREADS) k_interaction_slice(pdhg_ctl_t* __restrict__ ctl,
                                                                   int nloc,
                                                                   const double* __restrict__ src,
-                                                                  int n_src,
-                                                                  size_t src_stride,
                                                                   const double* __restrict__ xbuf0,
                                                                   const double* __restrict__ xbuf1,
                                                                   double* __restrict__ aty0,
@@ -807,16 +739,10 @@ __global__ void __launch_bounds__(EW_THREADS) k_interaction_slice(pdhg_ctl_t* __
                                                                   double* __restrict__ parts,
                                                                   const double* __restrict__ part_dy2,
                                                                   int n_part_dy2,
-                                                                  const unsigned long long* wait_flags,
-                                                                  peer_ptrs_t scal_peers,
-                                                                  peer_flags_t flags,
-                                                                  int world_out,
-                                                                  int rank)
+                                                                  double* __restrict__ scal)
 {
   if (!ctl->active) return;
   __shared__ double red[32];
-  const unsigned long long epoch = (unsigned long long)ctl->attempts + 1ull;
-  if (wait_flags) peer_wait(wait_flags, n_src, epoch);
   const int cur     = ctl->parity;
   const double* x   = cur ? xbuf1 : xbuf0;
   const double* xn  = cur ? xbuf0 : xbuf1;
@@ -825,8 +751,8 @@ __global__ void __launch_bounds__(EW_THREADS) k_interaction_slice(pdhg_ctl_t* __
   double acc[2]     = {0.0, 0.0};
   const int stride  = gridDim.x * blockDim.x;
   for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < nloc; j += stride) {
-    double s = 0.0;
-    for (int g = 0; g < n_src; ++g) s += __ldcg(src + (size_t)g * src_stride + j);
+    double s = 0.0;  // a sum from +0.0, not a copy: -0.0 becomes +0.0, and the iterates depend on the sign of a zero
+    s += __ldcg(src + j);
     atyn[j]        = s;
     const double d = xn[j] - x[j];
     acc[0] += d * (s - aty[j]);
@@ -837,19 +763,9 @@ __global__ void __launch_bounds__(EW_THREADS) k_interaction_slice(pdhg_ctl_t* __
   const double dx2         = gather_partials(parts + gridDim.x, gridDim.x, red);
   const double dy2         = gather_partials(part_dy2, n_part_dy2, red);
   if (threadIdx.x != 0) return;
-#pragma unroll
-  for (int r = 0; r < DIST_MAX_PEERS; ++r)
-    if (r < world_out) {
-      double* o = scal_peers.p[r];
-      o[0]      = interaction;
-      o[1]      = dx2;
-      o[2]      = dy2;
-    }
-  if (flags.p[0] == nullptr) return;
-  __threadfence_system();
-#pragma unroll
-  for (int r = 0; r < DIST_MAX_PEERS; ++r)
-    if (r < world_out) st_release_sys(flags.p[r] + DIST_FLAG_SCALARS + rank, epoch);
+  scal[0] = interaction;
+  scal[1] = dx2;
+  scal[2] = dy2;
 }
 
 // Step rule from the n_src scalar triples (rank order).  One warp.
@@ -878,7 +794,7 @@ __global__ void k_step_rule_gather(pdhg_ctl_t* __restrict__ ctl, const double* _
 // ---------------------------------------------------------------------------------------------
 // t[r] = (first ? 0 : t[r]) + sum over the entries of row r in this column block.
 //   pick_candidate = 0: x = x0;  1: x = the candidate dual y' = parity ? x0 : x1  (K3).
-//   wait_flags: peer transport only, first pass of K2 (the xbar slices of the other ranks must have landed).
+//   wait_flags: gather transport only, first pass of K2 / K3 (the other ranks' xbar / y' entries must have landed).
 __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_block_pass(const pdhg_ctl_t* __restrict__ ctl,
                                                                               bicsr_view_t Ab,
                                                                               const double* __restrict__ x0,
@@ -904,30 +820,6 @@ __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_block_pass(co
   };
   auto row_op = [&](int r, double s, const payload_t&) { st_l2(t + r, s, pol.stream); };
   spmv_bicsr_rows<payload_t, true>(Ab, x, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
-}
-
-// Peer transport, blocked K3p: t = partial A_g^T y'_g over all n columns -> staging rows of the slice owners.
-__global__ void __launch_bounds__(EW_THREADS) k_scatter_partials(pdhg_ctl_t* __restrict__ ctl,
-                                                                 int n,
-                                                                 const double* __restrict__ t,
-                                                                 peer_ptrs_t stage_peers,
-                                                                 int nslice,
-                                                                 peer_flags_t flags,
-                                                                 int world,
-                                                                 int rank)
-{
-  if (!ctl->active) return;
-  const unsigned long long epoch = (unsigned long long)ctl->attempts + 1ull;
-  const int stride               = gridDim.x * blockDim.x;
-  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += stride) {
-    const int h  = j / nslice;
-    double* base = stage_peers.p[0];
-#pragma unroll
-    for (int r = 1; r < DIST_MAX_PEERS; ++r)
-      if (h == r) base = stage_peers.p[r];
-    base[j - h * nslice] = __ldcs(t + j);
-  }
-  peer_signal_grid_done(&ctl->ticket[2], flags, world, DIST_FLAG_PARTIAL + rank, epoch);
 }
 
 // Applies a still-pending running-average update (end of a batch, before averages are formed).

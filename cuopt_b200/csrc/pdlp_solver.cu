@@ -333,17 +333,14 @@ struct pdlp_solver_t::impl_t {
   dvec<double> c, l, u, lc, uc, cs, ls, us, lcs, ucs, Dr, Dc;
   dvec<double> xbuf[2], ybuf[2], atybuf[2], xbar, sum_x, sum_y, x_avg, y_avg, x_lr, y_lr, rc_cur, rc_avg;
   dvec<double> part_dy2, part_k3, part_rows, part_cols, part_misc, scratch_n, scratch_m, d_scalar;
-  dvec<double> dist_buf;  // row-sharded mode: partial A^T y' (+1 slot) / 2n for the evaluation, all-reduced in place
+  dvec<double> dist_buf;  // sharded: partial A^T y' of the NCCL transport / 2n for the evaluation, summed over the ranks
   const dist_context_t* dist = nullptr;
   bool sharded() const { return dist != nullptr && dist->world > 1; }
-  // Transport of the sharded PDHG attempt (DESIGN.md §6): 0 = replicated primal side + one all-reduce (scheme (i)),
-  // 1 = column slices + NCCL all-gather / reduce-scatter (scheme (ii)), 2 = column slices + NVLink peer stores
-  // issued by the producing kernels (scheme (ii), no NCCL in the loop), 3 = "gather" (default): every rank also owns the
-  // rows J_g of the global A^T, so BOTH products take all-gathered inputs (xbar from K1, y' from K2, by peer stores) and
-  // there are no partial products at all.  CUOPT_B200_DIST_MODE=allreduce|nccl|p2p|gather.
-  enum { DIST_ALLREDUCE = 0, DIST_NCCL_SLICES = 1, DIST_P2P = 2, DIST_GATHER = 3 };
-  int dist_mode = DIST_ALLREDUCE;
-  bool peer_transport() const { return dist_mode == DIST_P2P || dist_mode == DIST_GATHER; }
+  // Transport of the sharded PDHG attempt (DESIGN.md §6), both on column slices (scheme (ii)); CUOPT_B200_DIST_MODE=gather|nccl.
+  // gather (default, dist_gather): every rank also owns the rows J_g of the global A^T, so BOTH products take all-gathered
+  // inputs (xbar from K1, y' from K2, by NVLink peer stores) and there are no partial products at all.
+  // nccl (also the fallback without peer access between the GPUs): NCCL all-gather of xbar, reduce-scatter of A_g^T y'.
+  bool dist_gather = false;
   // gather transport: global row offsets of the ranks, the all-gathered y', this rank's rows of the global scaled A^T
   int row0[DIST_MAX_PEERS + 1] = {};
   int m_total = 0;
@@ -369,7 +366,7 @@ struct pdlp_solver_t::impl_t {
   cudaStream_t comm_stream = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
   int grid_send = 1, send_slots = 0;  // SpMV CTA slots left to the send kernel (default: one per SM); CUOPT_B200_DIST_SEND_SLOTS
-  const csr_dev_t& hot_A() const { return (dist != nullptr && dist->world > 1 && dist_mode == DIST_GATHER) ? Ahot : As; }
+  const csr_dev_t& hot_A() const { return dist_gather ? Ahot : As; }
   // CUOPT_B200_DIST_TRACE=1: CUDA-event time of every kernel slot of the sharded attempt (waiting for the peers' flags
   // included), printed per rank when the solver goes away.  Turns the CUDA graphs off and synchronises once per attempt.
   bool dist_trace = false;
@@ -392,14 +389,13 @@ struct pdlp_solver_t::impl_t {
     ++tr_count;
   }
   int nslice = 0, n_pad = 0, slice_j0 = 0, slice_n = 0, grid_slice = 1;
-  dvec<double> rs_buf, stage, scal;
+  dvec<double> rs_buf, scal;
   dvec<unsigned long long> d_flags;
   void* xbar_peer[DIST_MAX_PEERS]  = {};
-  void* stage_peer[DIST_MAX_PEERS] = {};
   void* scal_peer[DIST_MAX_PEERS]  = {};
   void* flag_peer[DIST_MAX_PEERS]  = {};
   bool peers_open = false;
-  peer_ptrs_t p_xbar{}, p_stage{}, p_scal{};
+  peer_ptrs_t p_xbar{}, p_scal{};
   peer_flags_t p_flags{};
   dvec<unsigned> d_ticket;
   dvec<pdhg_ctl_t> d_ctl;
@@ -461,7 +457,6 @@ struct pdlp_solver_t::impl_t {
     if (!peers_open) return;
     cudaStreamSynchronize(stream);
     dist->close_peers(xbar_peer);
-    dist->close_peers(stage_peer);
     dist->close_peers(scal_peer);
     dist->close_peers(flag_peer);
     dist->close_peers(yfull_peer);
@@ -480,8 +475,8 @@ struct pdlp_solver_t::impl_t {
                    a.n_malloc, 1e3 * a.malloc_s, a.bytes * 1e-9, a.n_free, 1e3 * a.free_s);
     }
     if (dist_trace && tr_count > 0)
-      std::fprintf(stderr, "[cuopt-b200 dist trace] rank %d of %d, mode %d, %ld attempts: K1 %.1f us, K2 %.1f us, K3 %.1f us, rule %.1f us "
-                   "(each slot includes the wait for the peers' flags)\n", dist->rank, dist->world, dist_mode, tr_count,
+      std::fprintf(stderr, "[cuopt-b200 dist trace] rank %d of %d, gather transport, %ld attempts: K1 %.1f us, K2 %.1f us, K3 %.1f us, rule %.1f us "
+                   "(each slot includes the wait for the peers' flags)\n", dist->rank, dist->world, tr_count,
                    1e3 * tr_acc[0] / tr_count, 1e3 * tr_acc[1] / tr_count, 1e3 * tr_acc[2] / tr_count, 1e3 * tr_acc[3] / tr_count);
     for (auto& e : tr_ev) if (e) cudaEventDestroy(e);
     if (ev_fork) cudaEventDestroy(ev_fork);
@@ -503,7 +498,7 @@ struct pdlp_solver_t::impl_t {
     // gather transport: a consumer may spin on flags the send kernel of THIS rank still has to raise, so that kernel must
     // always find room beside a full wave of SpMV CTAs: send_slots CTA slots stay free (wherever the scheduler leaves them: each
     // holds >= 16 K registers = 2 send CTAs of 256 threads x 28 registers, and the send grid is 2 x send_slots CTAs)
-    const int reserve = (dist != nullptr && dist->world > 1 && dist_mode == DIST_GATHER && dist_send_kernel) ? send_slots : 0;
+    const int reserve = (dist_gather && dist_send_kernel) ? send_slots : 0;
     const int wave    = std::max(1, sms * (npre > 1 ? occ_spmv2 : occ_spmv) - reserve);
     return std::max(1, std::min((M.n_blk() + BICSR_WARPS - 1) / BICSR_WARPS, wave));
   }
@@ -701,14 +696,11 @@ struct pdlp_solver_t::impl_t {
   {
     dist_buf.resize(2 * (size_t)std::max(n, n_pad) + 8);
     dist_buf.zero(stream);
-    dist_mode = DIST_GATHER;
+    dist_gather = true;
     if (const char* e = std::getenv("CUOPT_B200_DIST_MODE")) {
       const std::string v(e);
-      if (v == "allreduce") dist_mode = DIST_ALLREDUCE;
-      else if (v == "nccl") dist_mode = DIST_NCCL_SLICES;
-      else if (v == "p2p") dist_mode = DIST_P2P;
-      else if (v == "gather") dist_mode = DIST_GATHER;
-      else throw lp_error(error_type_t::InvalidArgument, "CUOPT_B200_DIST_MODE must be allreduce, nccl, p2p or gather");
+      if (v == "nccl") dist_gather = false;
+      else if (v != "gather") throw lp_error(error_type_t::InvalidArgument, "CUOPT_B200_DIST_MODE must be gather or nccl");
     }
     {  // global row offsets of the ranks (the row blocks are contiguous and in rank order)
       dvec<double> cnt((size_t)dist->world);
@@ -727,46 +719,40 @@ struct pdlp_solver_t::impl_t {
     grid_slice = ew_grid(std::max(nslice, 1), sms);
     scal.resize(4 * DIST_MAX_PEERS);
     scal.zero(stream);
-    if (dist_mode == DIST_NCCL_SLICES) { rs_buf.resize(nslice); rs_buf.zero(stream); }
-    if (peer_transport()) {
-      if (dist_mode == DIST_P2P) stage.resize((size_t)nslice * dist->world);
-      else {
-        stage.resize(32);
-        yfull.resize((size_t)m_total + 64 * (size_t)dist->world + 64);
-        yfull.zero(stream);
-        xloc.resize((size_t)std::max(nslice, 32));
-        xloc.zero(stream);
-      }
-      stage.zero(stream);
+    if (dist_gather) {
+      yfull.resize((size_t)m_total + 64 * (size_t)dist->world + 64);
+      yfull.zero(stream);
+      xloc.resize((size_t)std::max(nslice, 32));
+      xloc.zero(stream);
       d_flags.resize(DIST_FLAG_COUNT);
       d_flags.zero(stream);
       // every rank's buffers are zeroed (stream order) before its handles leave through the stream-ordered all-gather
       bool ok = dist->open_peers(xbar.data(), xbar_peer, stream);
-      ok      = ok && dist->open_peers(stage.data(), stage_peer, stream);
       ok      = ok && dist->open_peers(scal.data(), scal_peer, stream);
       ok      = ok && dist->open_peers(d_flags.data(), flag_peer, stream);
-      if (dist_mode == DIST_GATHER) ok = ok && dist->open_peers(yfull.data(), yfull_peer, stream);
+      ok      = ok && dist->open_peers(yfull.data(), yfull_peer, stream);
       if (!ok) {  // unanimous (open_peers agrees across ranks): no peer access on this box -> NCCL transport
-        dist->close_peers(xbar_peer); dist->close_peers(stage_peer); dist->close_peers(scal_peer);
-        dist->close_peers(flag_peer); dist->close_peers(yfull_peer);
-        dist_mode = DIST_NCCL_SLICES;
-        rs_buf.resize(nslice);
-        rs_buf.zero(stream);
+        dist->close_peers(xbar_peer); dist->close_peers(scal_peer); dist->close_peers(flag_peer); dist->close_peers(yfull_peer);
+        dist_gather = false;
       } else {
         peers_open = true;
         for (int r = 0; r < dist->world; ++r) {
-          p_xbar.p[r]  = static_cast<double*>(xbar_peer[r]) + (dist_mode == DIST_GATHER ? 0 : slice_j0);
-          p_stage.p[r] = static_cast<double*>(stage_peer[r]) + (size_t)dist->rank * nslice;
+          p_xbar.p[r]  = static_cast<double*>(xbar_peer[r]);
           p_scal.p[r]  = static_cast<double*>(scal_peer[r]) + 4 * dist->rank;
           p_flags.p[r] = static_cast<unsigned long long*>(flag_peer[r]);
-          if (dist_mode == DIST_GATHER) p_yfull.p[r] = static_cast<double*>(yfull_peer[r]);
+          p_yfull.p[r] = static_cast<double*>(yfull_peer[r]);
         }
       }
+    }
+    if (!dist_gather) {
+      rs_buf.resize(nslice);
+      rs_buf.zero(stream);
+      use_graphs = false;  // NCCL calls between the kernels
     }
     if (const char* e = std::getenv("CUOPT_B200_DIST_TRACE")) dist_trace = e[0] == '1';
     if (const char* e = std::getenv("CUOPT_B200_DIST_PACK")) dist_pack = e[0] != '0';
     if (const char* e = std::getenv("CUOPT_B200_DIST_SEND")) dist_send_kernel = std::string(e) == "kernel";
-    if (dist_mode == DIST_GATHER) {
+    if (dist_gather) {
       CUOPT_CUDA_TRY(cudaStreamCreateWithFlags(&comm_stream, cudaStreamNonBlocking));
       CUOPT_CUDA_TRY(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
       CUOPT_CUDA_TRY(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
@@ -777,10 +763,6 @@ struct pdlp_solver_t::impl_t {
     if (dist_trace) {
       use_graphs = false;
       for (auto& e : tr_ev) CUOPT_CUDA_TRY(cudaEventCreate(&e));
-    }
-    if (!peer_transport()) {
-      use_graphs  = false;  // NCCL calls between the kernels
-      p_scal.p[0] = scal.data();
     }
   }
 
@@ -890,7 +872,7 @@ struct pdlp_solver_t::impl_t {
     fill_bicsr_values(As, stream, sms);
     fill_bicsr_values(ATs, stream, sms);
     trace.mark("scale problem + scaled BICSR values");
-    if (sharded() && dist_mode == DIST_GATHER) {
+    if (dist_gather) {
       build_gather_transport();  // packed A_g, rows J_g of the global A^T; the hot loop never multiplies by A_g^T
     } else {
       build_gather_blocks(As, blkA, t_m, 0, sharded() ? nullptr : &A);
@@ -1312,12 +1294,11 @@ struct pdlp_solver_t::impl_t {
   {
     const int k2 = blkA.on() ? blkA.B : 1;
     if (!sharded()) return 1 + k2 + (blkAT.on() ? blkAT.B : 1);
-    if (dist_mode == DIST_GATHER) return 1 + k2 + (blkATslice.on() ? blkATslice.B : 1) + 1 + (dist_send_kernel ? 2 : 0);
-    const int k3p = blkAT.on() ? blkAT.B + (dist_mode == DIST_P2P ? 1 : 0) : 1;
-    return 1 + k2 + k3p + (dist_mode == DIST_ALLREDUCE ? 2 : 2);
+    if (dist_gather) return 1 + k2 + (blkATslice.on() ? blkATslice.B : 1) + 1 + (dist_send_kernel ? 2 : 0);
+    return 1 + k2 + (blkAT.on() ? blkAT.B : 1) + 2;
   }
 
-  // partial A_g^T y' of this rank into dist_buf (NCCL transports); wide blocks when the shard's transpose is very sparse
+  // partial A_g^T y' of this rank into dist_buf (NCCL transport); wide blocks when the shard's transpose is very sparse
   void launch_transpose_partial()
   {
     if (blkAT.on()) {  // the passes accumulate straight into the collective's send buffer
@@ -1350,7 +1331,7 @@ struct pdlp_solver_t::impl_t {
   {
     const int j0 = slice_j0, G = dist->world, rk = dist->rank;
     double *x0 = xbuf[0].data() + j0, *x1 = xbuf[1].data() + j0, *a0 = atybuf[0].data() + j0, *a1 = atybuf[1].data() + j0;
-    if (dist_mode == DIST_GATHER) {
+    if (dist_gather) {
       const unsigned long long* fl = d_flags.data();
       tr_tick(0);
       if (dist_send_kernel) {
@@ -1376,7 +1357,7 @@ struct pdlp_solver_t::impl_t {
         CUOPT_CUDA_TRY(cudaStreamWaitEvent(comm_stream, ev_fork, 0));
         k_send_packed<<<grid_send, EW_THREADS, 0, comm_stream>>>(d_ctl.data(), ybuf[0].data(), ybuf[1].data(), 1, listY.data(),
                                                                  sendY.data(), m, planY, p_yfull, p_flags, G, rk,
-                                                                 DIST_FLAG_PARTIAL, DIST_FLAG_Y_B, d_ticket.data() + 4);
+                                                                 DIST_FLAG_Y, DIST_FLAG_Y_B, d_ticket.data() + 4);
         CUOPT_CUDA_TRY(cudaEventRecord(ev_join, comm_stream));
       }
       // K3 on this rank's rows of the global A^T, gathering from the packed y'; its last CTA sends this rank's three scalars
@@ -1384,7 +1365,7 @@ struct pdlp_solver_t::impl_t {
       const csr_dev_t& L = blocked ? blkATslice.blk[blkATslice.B - 1] : ATslice;
       const int grid     = spmv_grid(L, 1);
       if (blocked)
-        launch_block_passes(blkATslice, blkATslice.B - 1, yfull.data(), yfull.data(), 0, t_slice.data(), fl + DIST_FLAG_PARTIAL, G);
+        launch_block_passes(blkATslice, blkATslice.B - 1, yfull.data(), yfull.data(), 0, t_slice.data(), fl + DIST_FLAG_Y, G);
 #define CUOPT_K3S(INIT)                                                                                                     \
   k_transpose_step_slice<INIT, 1><<<grid, BICSR_THREADS, 0, stream>>>(                                                      \
     d_ctl.data(), L.view(), yfull.data(), x0, x1, a0, a1, part_k3.data(), part_dy2.data(), n_part_dy2,                      \
@@ -1398,29 +1379,6 @@ struct pdlp_solver_t::impl_t {
       tr_close(4);
       return;
     }
-    if (dist_mode == DIST_P2P) {
-      tr_tick(0);
-      k_primal_step_bcast<<<grid_slice, EW_THREADS, 0, stream>>>(d_ctl.data(), slice_n, x0, x1, a0, a1, cs.data() + j0,
-                                                                 ls.data() + j0, us.data() + j0, sum_x.data() + j0, p_xbar,
-                                                                 p_flags, G, rk);
-      tr_tick(1);
-      enqueue_k2(d_flags.data() + DIST_FLAG_XBAR, G);
-      tr_tick(2);
-      if (blkAT.on()) {
-        launch_block_passes(blkAT, blkAT.B, ybuf[0].data(), ybuf[1].data(), 1, t_n.data(), nullptr, 0);
-        k_scatter_partials<<<grid_n, EW_THREADS, 0, stream>>>(d_ctl.data(), n, t_n.data(), p_stage, nslice, p_flags, G, rk);
-      } else
-        k_transpose_partial_scatter<<<grid_k3, BICSR_THREADS, 0, stream>>>(d_ctl.data(), ATs.view(), ybuf[0].data(),
-                                                                          ybuf[1].data(), p_stage, nslice, p_flags, G, rk);
-      k_interaction_slice<<<grid_slice, EW_THREADS, 0, stream>>>(d_ctl.data(), slice_n, stage.data(), G, (size_t)nslice, x0, x1,
-                                                                 a0, a1, part_k3.data(), part_dy2.data(), n_part_dy2,
-                                                                 d_flags.data() + DIST_FLAG_PARTIAL, p_scal, p_flags, G, rk);
-      tr_tick(3);
-      k_step_rule_gather<<<1, 32, 0, stream>>>(d_ctl.data(), scal.data(), G, d_flags.data() + DIST_FLAG_SCALARS);
-      tr_tick(4);
-      tr_close(4);
-      return;
-    }
     k_primal_step<<<grid_slice, EW_THREADS, 0, stream>>>(d_ctl.data(), slice_n, x0, x1, a0, a1, cs.data() + j0,
                                                          ls.data() + j0, us.data() + j0, sum_x.data() + j0,
                                                          xbar.data() + j0);
@@ -1428,17 +1386,15 @@ struct pdlp_solver_t::impl_t {
     enqueue_k2(nullptr, 0);
     launch_transpose_partial();
     dist->reduce_scatter(dist_buf.data(), rs_buf.data(), nslice, stream);
-    peer_flags_t no_flags{};
-    k_interaction_slice<<<grid_slice, EW_THREADS, 0, stream>>>(d_ctl.data(), slice_n, rs_buf.data(), 1, 0, x0, x1, a0, a1,
-                                                               part_k3.data(), part_dy2.data(), n_part_dy2, nullptr, p_scal,
-                                                               no_flags, 1, rk);
+    k_interaction_slice<<<grid_slice, EW_THREADS, 0, stream>>>(d_ctl.data(), slice_n, rs_buf.data(), x0, x1, a0, a1,
+                                                               part_k3.data(), part_dy2.data(), n_part_dy2, scal.data());
     dist->allreduce(scal.data(), 3, false, stream);
     k_step_rule_gather<<<1, 32, 0, stream>>>(d_ctl.data(), scal.data(), 1, nullptr);
   }
 
   void enqueue_attempt()
   {
-    if (sharded() && dist_mode != DIST_ALLREDUCE) {
+    if (sharded()) {
       enqueue_sliced_attempt();
       return;
     }
@@ -1446,16 +1402,7 @@ struct pdlp_solver_t::impl_t {
                                                       atybuf[1].data(), cs.data(), ls.data(), us.data(), sum_x.data(),
                                                       xbar.data());
     enqueue_k2(nullptr, 0);
-    if (!sharded()) {
-      enqueue_k3();
-      return;
-    }
-    // row-sharded: partial A_g^T y'_g and this rank's ||dy||^2 -> one all-reduce of n + 1 doubles -> K3b
-    launch_transpose_partial();
-    k_sum_partials<<<1, EW_THREADS, 0, stream>>>(d_ctl.data(), part_dy2.data(), n_part_dy2, 1, dist_buf.data() + n);
-    dist->allreduce(dist_buf.data(), (size_t)n + 1, false, stream);
-    k_interaction_step<<<grid_n, EW_THREADS, 0, stream>>>(d_ctl.data(), n, dist_buf.data(), xbuf[0].data(), xbuf[1].data(),
-                                                          atybuf[0].data(), atybuf[1].data(), part_k3.data());
+    enqueue_k3();
   }
 
   void launch_attempts(int count)
@@ -1511,8 +1458,7 @@ struct pdlp_solver_t::impl_t {
     while (true) {
       // a couple of spare attempts cover the occasional rejected step without another round trip
       launch_attempts(todo + (todo >= 16 ? 2 : 0));
-      const bool sliced = sharded() && dist_mode != DIST_ALLREDUCE;
-      const int fj0 = sliced ? slice_j0 : 0, fn = sliced ? slice_n : n;
+      const int fj0 = sharded() ? slice_j0 : 0, fn = sharded() ? slice_n : n;
       k_flush_average<<<grid_misc, EW_THREADS, 0, stream>>>(d_ctl.data(), fn, xbuf[0].data() + fj0, xbuf[1].data() + fj0,
                                                             sum_x.data() + fj0, m, ybuf[0].data(), ybuf[1].data(),
                                                             sum_y.data());
@@ -1523,7 +1469,7 @@ struct pdlp_solver_t::impl_t {
       if (h_ctl->valid == -1 || h_ctl->accepted >= target) break;
       todo = target - h_ctl->accepted;
     }
-    if (sharded() && dist_mode != DIST_ALLREDUCE) {
+    if (sharded()) {
       // back to the replicated representation the major-iteration code works on: every rank receives the other
       // slices of the current iterate, its A^T y and the running sum (3 all-gathers per batch of ~40 attempts)
       const int cur = h_ctl->parity;
@@ -1583,7 +1529,7 @@ struct pdlp_solver_t::impl_t {
       const double* rows_src  = part_rows.data();
       int rows_count          = n_rows_parts;
       if (sharded()) {
-        k_sum_partials<<<1, EW_THREADS, 0, stream>>>(nullptr, part_rows.data(), n_rows_parts, 6, d_scalar.data());
+        k_sum_partials<<<1, EW_THREADS, 0, stream>>>(part_rows.data(), n_rows_parts, 6, d_scalar.data());
         dist->allreduce(d_scalar.data(), 6, false, stream);
         rows_src   = d_scalar.data();
         rows_count = 1;

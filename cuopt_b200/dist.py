@@ -80,7 +80,7 @@ def reference_protocol_step_sliced(shard, rank, world, x_slice, x_next_slice, at
                                    allgather, reduce_scatter_sum, allgather_scalars):
     """One attempt of the column-sliced scheme (DESIGN.md §6, scheme (ii)) in numpy: this rank holds rows R_g of A and
     the slice J_g of x, x', A^T y.  Exchanges: xbar slices -> everyone; partial A_g^T y'_g -> slice owners (summed in
-    RANK ORDER, as the peer-store transport does); three scalars per rank -> everyone (summed in rank order).
+    RANK ORDER); three scalars per rank -> everyone (summed in rank order).
     Returns (y_next_local, aty_next_slice, interaction, ||dx||^2, ||dy||^2) with the scalars identical on all ranks."""
     A = shard
     n = A.shape[1]

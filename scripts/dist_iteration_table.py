@@ -21,7 +21,7 @@ def main():
             s1, s2 = one.stats(), two.stats()
             print(f"tol {tol:g} mode {mode}: single its {s1.number_of_steps_taken} / {s2.number_of_steps_taken} obj "
                   f"{s1.primal_objective:.9g} planted {lp.optimal_objective:.9g}", flush=True)
-            for tr in (("nccl", "p2p") if quick else ("allreduce", "nccl", "p2p")):
+            for tr in ("gather", "nccl"):
                 r = T._solve_on_gpus(world, size, tol, mode, tr)
                 print(f"    {tr:10s} its {r[0]['its']} obj {r[0]['obj']:.9g} dobj {r[0]['dobj']:.9g} status {r[0]['status']}",
                       flush=True)

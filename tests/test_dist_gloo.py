@@ -11,7 +11,8 @@
     oracle's own twenty steps (same accept / reject decisions on every rank, iterates to 1e-10),
   * the packed exchange (two halves, slot tables, send lists) delivers exactly what every rank reads,
   * the slice bounds tile [0, n) with 32-aligned slices.
-The CUDA side of the same protocols is exercised by tests/test_gpu_dist.py on >= 2 GPUs."""
+Two of these protocols run in CUDA: the gather transport, and the column-sliced scheme as the nccl transport.
+tests/test_gpu_dist.py exercises both on >= 2 GPUs; the one-all-reduce attempt is a CPU model only."""
 import os
 import socket
 

@@ -40,16 +40,19 @@ def _worker(rank, world, port, q, size, extra_cols, tol, mode, transport, block_
             s.set("iteration_limit", iteration_limit)
         s.set("optimality_tolerance", tol)
         sol = capi.solve_distributed(p, s, comm)
-        st = sol.stats()
-        q.put(dict(rank=rank, rc=sol.return_code, err=sol.error_string, status=sol.termination_status,
-                   its=st.number_of_steps_taken, obj=st.primal_objective, dobj=st.dual_objective, x=sol.primal(),
-                   y=sol.dual(), rows=(r0, r1), rp=st.l2_primal_residual))
+        out = dict(rank=rank, rc=sol.return_code, err=sol.error_string)
+        if sol.return_code == 0:
+            st = sol.stats()
+            out.update(status=sol.termination_status, its=st.number_of_steps_taken, obj=st.primal_objective,
+                       dobj=st.dual_objective, x=sol.primal(), y=sol.dual(), rows=(r0, r1), rp=st.l2_primal_residual)
+        q.put(out)
         dist.barrier()
     finally:
         dist.destroy_process_group()
 
 
-def _solve_on_gpus(world, size, tol, mode, transport, extra_cols=0, block_bytes=0, iteration_limit=0, nnz_per_row=8):
+def _solve_on_gpus(world, size, tol, mode, transport, extra_cols=0, block_bytes=0, iteration_limit=0, nnz_per_row=8,
+                   expect_ok=True):
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
@@ -67,6 +70,8 @@ def _solve_on_gpus(world, size, tol, mode, transport, extra_cols=0, block_bytes=
         for p in procs:  # a rank that trapped or hung must not outlive the test
             if p.is_alive():
                 p.kill()
+    if not expect_ok:
+        return res
     for r in res:
         assert r["rc"] == 0, r["err"]
     # every rank reports the same status / iteration count / objectives / primal vector (identical decisions everywhere)
@@ -90,11 +95,11 @@ def _single_gpu(size, tol, mode, iteration_limit=0, nnz_per_row=8, extra_cols=0)
     return lp, one
 
 
-@pytest.mark.parametrize("transport,nnz_per_row", [("gather", 8), ("gather", 2), ("gather-nopack", 2), ("gather-kernel", 8), ("gather-kernel", 2), ("p2p", 8), ("nccl", 8)])
+@pytest.mark.parametrize("transport,nnz_per_row", [("gather", 8), ("gather", 2), ("gather-nopack", 2), ("gather-kernel", 8), ("gather-kernel", 2), ("nccl", 8), ("nccl", 2)])
 def test_sharded_iterates_track_the_single_gpu_iterates(transport, nnz_per_row):
     """The strongest check of a transport: after the SAME number of iterations (no tolerance involved) the sharded solve holds
     the iterate the single GPU holds, element-wise, up to the summation order of the row sums (block cuts of the row blocks
-    differ from those of the whole matrix; p2p / nccl also add the partial A_g^T y' in rank order).  A stale or torn xbar / y'
+    differ from those of the whole matrix; nccl also adds the partial A_g^T y' over the ranks).  A stale or torn xbar / y'
     exchange shows up here as an O(1) difference.  The 2-per-row LP makes every rank need only part of the other ranks' slices."""
     import torch
     if torch.cuda.device_count() < 2:
@@ -115,9 +120,10 @@ def test_sharded_iterates_track_the_single_gpu_iterates(transport, nnz_per_row):
 
 
 # transport of the sharded attempt: gather = every rank owns rows of A AND rows of the global A^T, both products take inputs
-# all-gathered by NVLink peer stores of the producing kernels (default); p2p = peer stores with partial A_g^T y' scattered to
-# the slice owners; nccl = all-gather + reduce-scatter; allreduce = replicated primal side (scheme (i))
-@pytest.mark.parametrize("mode,transport", [(1, "gather"), (1, "p2p"), (1, "nccl"), (1, "allreduce"), (3, "gather"), (3, "p2p")])
+# all-gathered by NVLink peer stores of the producing kernels (default; -kernel: k_send_packed, -nopack: every entry
+# travels); nccl = all-gather + reduce-scatter
+@pytest.mark.parametrize("mode,transport", [(1, "gather"), (1, "gather-kernel"), (1, "gather-nopack"), (1, "nccl"), (3, "gather"),
+                                            (3, "nccl")])
 def test_two_gpu_solve_matches_single_gpu(mode, transport):
     import torch
     if torch.cuda.device_count() < 2:
@@ -146,15 +152,15 @@ def test_two_gpu_solve_matches_single_gpu(mode, transport):
 
 @pytest.mark.parametrize("world", [4, 8])
 def test_four_and_eight_gpu_solve_matches_single_gpu(world):
-    """The same comparison on 4 and 8 ranks (peer-store transport; slices of 1/4 and 1/8 of the columns, rank-ordered sums of
-    4 / 8 partials): needs 4 / 8 GPUs, skipped on smaller machines."""
+    """The same comparison on 4 and 8 ranks (both transports; slices of 1/4 and 1/8 of the columns): needs 4 / 8 GPUs,
+    skipped on smaller machines."""
     import torch
     if torch.cuda.device_count() < world:
         pytest.skip(f"needs {world} GPUs")
     size, tol = 40_000, 1e-6
     lp, one = _single_gpu(size, tol, 1)
     st1 = one.stats()
-    for transport in ("gather", "p2p"):
+    for transport in ("gather", "nccl"):
         res = _solve_on_gpus(world, size, tol, 1, transport)
         assert res[0]["status"] == 1
         assert res[0]["obj"] == pytest.approx(lp.optimal_objective, rel=1e-5)
@@ -183,24 +189,20 @@ def test_many_gpu_iterates_track_the_single_gpu_iterates(world):
     assert res[0]["obj"] == pytest.approx(one.stats().primal_objective, rel=1e-7, abs=1e-7)
 
 
-def test_peer_store_transport_is_deterministic_and_equals_nccl_transport():
-    """With two ranks a + b == b + a, so the peer-store transport (rank-ordered sums) and the NCCL transport must
-    produce bit-identical iterates; and the peer-store transport must reproduce itself run to run (no race between the
-    NVLink stores, the flags and the consuming kernels)."""
+def test_nccl_transport_is_deterministic_with_ragged_slices():
+    """The NCCL transport reproduces itself bit for bit, also when the last column slice is shorter than the 32-aligned
+    slice width."""
     import torch
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     size, tol, world = 40_000, 1e-6, 2
     ragged = 37  # n = 40037: the last slice is shorter than the 32-aligned slice width
-    a = _solve_on_gpus(world, size, tol, 1, "p2p", ragged)
-    b = _solve_on_gpus(world, size, tol, 1, "p2p", ragged)
-    c = _solve_on_gpus(world, size, tol, 1, "nccl", ragged)
+    a = _solve_on_gpus(world, size, tol, 1, "nccl", ragged)
+    b = _solve_on_gpus(world, size, tol, 1, "nccl", ragged)
     assert a[0]["status"] == 1
-    for other in (b, c):
-        assert other[0]["its"] == a[0]["its"]
-        assert other[0]["obj"] == a[0]["obj"] and other[0]["dobj"] == a[0]["dobj"]
-        assert np.array_equal(other[0]["x"], a[0]["x"])
-        assert all(np.array_equal(other[r]["y"], a[r]["y"]) for r in range(world))
+    assert b[0]["its"] == a[0]["its"] and b[0]["obj"] == a[0]["obj"] and b[0]["dobj"] == a[0]["dobj"]
+    assert np.array_equal(b[0]["x"], a[0]["x"])
+    assert all(np.array_equal(b[r]["y"], a[r]["y"]) for r in range(world))
 
 
 def test_gather_transport_is_deterministic_with_ragged_slices():
@@ -218,7 +220,7 @@ def test_gather_transport_is_deterministic_with_ragged_slices():
     assert all(np.array_equal(b[r]["y"], a[r]["y"]) for r in range(world))
 
 
-@pytest.mark.parametrize("transport", ["gather", "p2p", "nccl"])
+@pytest.mark.parametrize("transport", ["gather", "gather-nopack", "nccl"])
 def test_two_gpu_solve_with_gather_blocking(transport):
     """The large-LP kernels (column-blocked passes + element-wise epilogues / scatter) inside the sharded attempt:
     forced on a small LP (4 blocks for A_g, 2 for A_g^T), they must reach the same optimum as the fused kernels."""
@@ -233,3 +235,17 @@ def test_two_gpu_solve_with_gather_blocking(transport):
     assert blocked[0]["obj"] == pytest.approx(fused[0]["obj"], rel=1e-3)  # both are tolerance-1e-4 points
     lp, one = _single_gpu(size, tol, 1)
     assert blocked[0]["obj"] == pytest.approx(lp.optimal_objective, rel=1e-3)
+
+
+def test_unknown_transport_is_rejected_on_every_rank():
+    """A transport name other than gather or nccl (here "p2p") is an invalid argument on every rank.  Each rank raises it
+    while it builds the solver, before the first collective, so no rank is left waiting for the others."""
+    import torch
+    from cuopt_b200 import capi
+    if torch.cuda.device_count() < 2:
+        pytest.skip("needs 2 GPUs")
+    res = _solve_on_gpus(2, 4_000, 1e-4, 1, "p2p", expect_ok=False)
+    assert len(res) == 2
+    for r in res:
+        assert r["rc"] == capi.CUOPT_INVALID_ARGUMENT
+        assert "gather" in r["err"] and "nccl" in r["err"]
