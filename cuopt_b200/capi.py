@@ -67,6 +67,7 @@ REFERENCE_SYMBOLS = [
 EXTENSION_SYMBOLS = [
     "cuOptB200GetLPStats", "cuOptB200SolverCreate", "cuOptB200SolverDestroy", "cuOptB200SolverInitialise",
     "cuOptB200SolverAdvance", "cuOptB200SolverGetScalar", "cuOptB200SolverGetVector", "cuOptB200SolverGetSolution",
+    "cuOptB200SolverTrustRegionBounds",
     "cuOptB200SolverProfileKernels", "cuOptB200ReadProblem", "cuOptB200Version", "cuOptB200DistGetUniqueId",
     "cuOptB200DistInit", "cuOptB200DistDestroy", "cuOptB200SolveDistributed",
     "cuOptB200SetWarmStartCapture", "cuOptB200GetWarmStart", "cuOptB200SetWarmStart", "cuOptB200CreateWarmStart",
@@ -149,6 +150,7 @@ def lib():
         L.cuOptB200SolverGetScalar.argtypes = [vp, C.c_char_p, c_dbl_p]
         L.cuOptB200SolverGetVector.argtypes = [vp, C.c_char_p, c_dbl_p, C.c_int32, c_int_p]
         L.cuOptB200SolverGetSolution.argtypes = [vp, C.POINTER(vp)]
+        L.cuOptB200SolverTrustRegionBounds.argtypes = [vp, c_dbl_p, c_dbl_p, C.c_double, c_dbl_p, c_dbl_p]
         L.cuOptB200SolverProfileKernels.argtypes = [vp, C.c_int32, C.c_int32, C.POINTER(KernelProfile)]
         L.cuOptB200ReadProblem.argtypes = [C.c_char_p, C.c_int32, C.POINTER(vp)]
         L.cuOptB200Version.restype = C.c_char_p
@@ -487,6 +489,16 @@ class Solver:
         out = np.zeros(sz.value)
         _check(lib().cuOptB200SolverGetVector(self.h, name.encode(), _dp(out), sz.value, C.byref(sz)), name)
         return out
+
+    def trust_region_bounds(self, px, py, radius: float):
+        """(lower, upper) of the Methodical1 trust-region restart at a point of the scaled space; changes no state."""
+        px = np.ascontiguousarray(px, np.float64); py = np.ascontiguousarray(py, np.float64)
+        if len(px) != self.n or len(py) != self.m:
+            raise ValueError(f"expected {self.n} primal and {self.m} dual values, got {len(px)} and {len(py)}")
+        lo, up = C.c_double(), C.c_double()
+        _check(lib().cuOptB200SolverTrustRegionBounds(self.h, _dp(px), _dp(py), float(radius), C.byref(lo), C.byref(up)),
+               "trust_region_bounds")
+        return lo.value, up.value
 
     def solution(self) -> Solution:
         h = C.c_void_p()

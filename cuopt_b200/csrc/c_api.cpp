@@ -777,6 +777,18 @@ cuopt_int_t cuOptB200SolverGetVector(cuOptB200Solver solver,
   });
   return CUOPT_SUCCESS;
 }
+cuopt_int_t cuOptB200SolverTrustRegionBounds(cuOptB200Solver solver,
+                                             const cuopt_float_t* px,
+                                             const cuopt_float_t* py,
+                                             cuopt_float_t radius,
+                                             cuopt_float_t* lower_ptr,
+                                             cuopt_float_t* upper_ptr)
+{
+  if (solver == nullptr || px == nullptr || py == nullptr || lower_ptr == nullptr || upper_ptr == nullptr)
+    return CUOPT_INVALID_ARGUMENT;
+  SOLVER_GUARD(static_cast<solver_handle_t*>(solver)->solver->trust_region_bounds(px, py, radius, *lower_ptr, *upper_ptr));
+  return CUOPT_SUCCESS;
+}
 cuopt_int_t cuOptB200SolverGetSolution(cuOptB200Solver solver, cuOptSolution* solution_ptr)
 {
   if (solver == nullptr || solution_ptr == nullptr) return CUOPT_INVALID_ARGUMENT;

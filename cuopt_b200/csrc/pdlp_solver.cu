@@ -1796,6 +1796,21 @@ struct pdlp_solver_t::impl_t {
     g.upper = h_scalar[1];
     launches += degenerate ? 4 : 6;
   }
+  // tr_bound at a caller-given point (cuOptB200SolverTrustRegionBounds).  Only the tr_* scratch buffers are written;
+  // the iterates, the restart state and the launch count are left as they were.
+  void trust_region_bounds_at(const double* hx, const double* hy, double radius, double& lower, double& upper)
+  {
+    dvec<double> px, py;
+    px.upload(hx, (size_t)n, stream);
+    py.upload(hy, (size_t)m, stream);
+    tr_gap_t g{px.data(), py.data()};
+    g.dist                = radius;
+    const long long count = launches;
+    tr_bound(g);  // ends with a stream sync: px / py may be freed afterwards
+    launches = count;
+    lower    = g.lower;
+    upper    = g.upper;
+  }
   void trust_region_restart()  // pdlp_restart_strategy.cu:278-364
   {
     nvtx_range_t nvtx_scope("run trust region restart");
@@ -2058,6 +2073,16 @@ std::vector<double> pdlp_solver_t::vector(const std::string& name)
   v->download(h.data(), s.stream);
   s.sync();
   return h;
+}
+
+void pdlp_solver_t::trust_region_bounds(const double* px, const double* py, double radius, double& lower, double& upper)
+{
+  impl_t& s = *impl_;
+  if (!s.tr_enabled) throw lp_error(error_type_t::InvalidArgument, "trust-region bounds need pdlp_solver_mode Methodical1");
+  if (!s.initialised) throw lp_error(error_type_t::InvalidArgument, "trust-region bounds need an initialised session");
+  if (!(radius >= 0.0)) throw lp_error(error_type_t::InvalidArgument, "trust-region radius must be >= 0");
+  s.fetch_ctl();
+  s.trust_region_bounds_at(px, py, radius, lower, upper);
 }
 
 kernel_profile_t pdlp_solver_t::profile_kernels(int warmup_steps, int reps)

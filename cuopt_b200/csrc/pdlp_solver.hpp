@@ -41,6 +41,9 @@ class pdlp_solver_t {
   double scalar(const std::string& name);
   std::vector<double> vector(const std::string& name);
   kernel_profile_t profile_kernels(int warmup_steps, int reps);
+  // Lower / upper bound of the trust-region restart (Methodical1) at a point (px: n, py: m values) of the scaled space,
+  // radius >= 0; reads the solver state, changes none of it.
+  void trust_region_bounds(const double* px, const double* py, double radius, double& lower, double& upper);
   const lp_solution_t& solution() const;
 
   struct impl_t;

@@ -87,6 +87,16 @@ cuopt_int_t cuOptB200SolverGetVector(cuOptB200Solver solver,
                                      cuopt_float_t* values,
                                      cuopt_int_t capacity,
                                      cuopt_int_t* size_ptr);
+/* Read-only: lower / upper bound of the trust-region restart of Methodical1 (bound_optimal_objective) at a point of
+ * the SCALED space (px: num_variables values, py: num_constraints values) for a radius >= 0, from the same kernels the
+ * restart runs.  The session must be initialised with pdlp_solver_mode Methodical1; its iterates, restart state and
+ * statistics are not changed. */
+cuopt_int_t cuOptB200SolverTrustRegionBounds(cuOptB200Solver solver,
+                                             const cuopt_float_t* px,
+                                             const cuopt_float_t* py,
+                                             cuopt_float_t radius,
+                                             cuopt_float_t* lower_ptr,
+                                             cuopt_float_t* upper_ptr);
 /* Solution object (same type cuOptSolve returns) of a finished session. */
 cuopt_int_t cuOptB200SolverGetSolution(cuOptB200Solver solver, cuOptSolution* solution_ptr);
 /* Time the three PDHG kernels in situ (CUDA events on the solver's stream) after `warmup_steps`. */
