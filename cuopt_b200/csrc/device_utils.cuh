@@ -68,6 +68,7 @@ class device_block_cache_t {
         void* p = blocks_[i].p;
         cached_ -= bytes;
         blocks_.erase(blocks_.begin() + (long)i);
+        ++hits_;
         return p;
       }
     return nullptr;
@@ -94,6 +95,12 @@ class device_block_cache_t {
         ++first_kept;
       }
     }
+  }
+  // requests served from the cache so far, all devices (read-only diagnostics)
+  long long hits()
+  {
+    std::lock_guard<std::mutex> g(mu_);
+    return hits_;
   }
   void flush()
   {
@@ -122,6 +129,7 @@ class device_block_cache_t {
   std::mutex mu_;
   std::vector<block_t> blocks_;
   size_t cached_ = 0, cap_ = 0;
+  long long hits_ = 0;
 };
 
 // Device array with value semantics disabled; one allocation per vector, sized once per solve, taken from / returned to the

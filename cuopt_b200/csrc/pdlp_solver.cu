@@ -268,8 +268,15 @@ class staged_uploader_t {
                       size_t(2) << 20);
       CUOPT_CUDA_TRY(cudaMemcpyAsync(to + done, slot, b, cudaMemcpyHostToDevice, s));
       CUOPT_CUDA_TRY(cudaEventRecord(free_[k], s));
+      ++fills_;
       done += b;
     }
+  }
+  // slot fills so far (a session reads it before and after its uploads: the plain path leaves it unchanged)
+  long long fills()
+  {
+    std::lock_guard<std::mutex> guard(mu_);
+    return fills_;
   }
 
  private:
@@ -279,6 +286,7 @@ class staged_uploader_t {
   char* buf_ = nullptr;
   bool tried_ = false;
   int next_ = 0;
+  long long fills_ = 0;
   cudaEvent_t free_[SLOTS] = {};
   bool ensure()
   {
@@ -433,6 +441,7 @@ struct pdlp_solver_t::impl_t {
   size_t gather_block_bytes = 0;  // set in build() from the device's L2 size (see there)
   int n_part_dy2 = 1;  // CTAs that publish ||dy||^2 partials: grid_k2 (fused K2) or grid_m (blocked K2 epilogue)
   int grid_k1 = 1, grid_k2 = 1, grid_k3 = 1, grid_n = 1, grid_m = 1, grid_misc = 1;
+  long long staged_fills = 0;  // staging-ring slot fills while this session uploaded (the ring is per device)
   std::map<int, cudaGraphExec_t> graphs;
   bool use_graphs = true;
   cudaEvent_t ev_a = nullptr, ev_b = nullptr;
@@ -554,6 +563,7 @@ struct pdlp_solver_t::impl_t {
     if (maximize) obj_scale = -obj_scale;
     trace.stream = stream;
     trace.mark("stream + pinned control buffers");
+    const long long fills0 = staged_uploader_t::get().fills();
     upload_csr(A, m, n, p.A_offsets, p.A_indices, p.A_values, stream, sms);
     trace.mark("upload A + BICSR(A)");
     transpose_to(AT, A, stream, sms);
@@ -597,6 +607,7 @@ struct pdlp_solver_t::impl_t {
       if (h_bad[0]) throw lp_error(error_type_t::ValidationError, "Variable lower bound above upper bound");
       if (h_bad[1]) throw lp_error(error_type_t::ValidationError, "Constraint lower bound above upper bound");
     }
+    staged_fills = staged_uploader_t::get().fills() - fills0;
     cs.copy_from(c, stream); ls.copy_from(l, stream); us.copy_from(u, stream); lcs.copy_from(lc, stream); ucs.copy_from(uc, stream);
     trace.mark("objective / bound vectors");
 
@@ -1273,12 +1284,14 @@ struct pdlp_solver_t::impl_t {
     return spmv_grid(L, fused_npre(L));
   }
   // K3 on one GPU: same structure, the step rule runs in the last CTA of the fused kernel
+  int k3_npre() const { return npre_override > 1 ? 2 : 1; }  // two payload sets pay in K2 only (fused_npre), not in this last pass
+  int k3_grid() const { return spmv_grid(blkAT.on() ? blkAT.blk[blkAT.B - 1] : ATs, k3_npre()); }
   void enqueue_k3()
   {
     const bool blocked = blkAT.on();
     const csr_dev_t& L = blocked ? blkAT.blk[blkAT.B - 1] : ATs;
-    const int npre     = npre_override > 1 ? 2 : 1;  // two payload sets pay in K2 only (fused_npre), not in this last pass
-    const int grid     = spmv_grid(L, npre);
+    const int npre     = k3_npre();
+    const int grid     = k3_grid();
     const double* t    = blocked ? t_n.data() : nullptr;
     if (blocked) launch_block_passes(blkAT, blkAT.B - 1, ybuf[0].data(), ybuf[1].data(), 1, t_n.data(), nullptr, 0);
 #define CUOPT_K3(INIT, NPRE)                                                                                              \
@@ -2037,6 +2050,23 @@ double pdlp_solver_t::scalar(const std::string& name)
   if (name == "eval_blocks") return (double)std::max<size_t>(1, s.blkA.unscaled.size());  // passes of the evaluation's A x
   if (name == "eval_blocks_t") return (double)std::max<size_t>(1, s.blkAT.unscaled.size());
   if (name == "valid") return k.valid;
+  // launch geometry (read-only): grid_k2 / grid_k3 as the fused K2 / K3 launch (on the last column block when blocked),
+  // n_std / n_blk of the whole scaled A and A^T
+  if (name == "sm_count") return s.sms;
+  if (name == "occ_spmv") return s.occ_spmv;
+  if (name == "occ_spmv2") return s.occ_spmv2;
+  if (name == "grid_k1") return s.grid_k1;
+  if (name == "grid_k2") return s.k2_grid();
+  if (name == "grid_k3") return s.k3_grid();
+  if (name == "grid_n") return s.grid_n;
+  if (name == "grid_m") return s.grid_m;
+  if (name == "k2_npre") return s.fused_npre(s.blkA.on() ? s.blkA.blk[s.blkA.B - 1] : s.hot_A());
+  if (name == "n_std_a") return s.As.bi_structure().n_std;
+  if (name == "n_blk_a") return s.As.bi_structure().n_blk;
+  if (name == "n_std_at") return s.ATs.bi_structure().n_std;
+  if (name == "n_blk_at") return s.ATs.bi_structure().n_blk;
+  if (name == "staged_fills") return (double)s.staged_fills;
+  if (name == "device_cache_hits") return (double)device_block_cache_t::get().hits();
   return std::nan("");
 }
 

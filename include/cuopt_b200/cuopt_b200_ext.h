@@ -78,6 +78,14 @@ cuopt_int_t cuOptB200SolverInitialise(cuOptB200Solver solver);
 cuopt_int_t cuOptB200SolverAdvance(cuOptB200Solver solver, cuopt_int_t accepted_steps, cuopt_int_t* finished_ptr);
 /* Named state: scalars "step_size", "primal_weight", "tau", "sigma", "sum_w", "k_total", "k_pdhg",
  * "its_since_restart", "interaction", "norm_dx2", "norm_dy2", "l2_norm_b", "l2_norm_c", "n_restarts";
+ * launch geometry (read-only): "sm_count", "occ_spmv" / "occ_spmv2" (resident CTAs per SM of the SpMV kernels with one /
+ * two payload row groups), "grid_k1", "grid_k2", "grid_k3" (CTAs of the primal step and of the fused K2 / K3 as they
+ * launch: on the last column block when gather blocking is on), "grid_n", "grid_m" (element-wise grids), "k2_npre"
+ * (payload row groups of the fused K2), "n_std_a", "n_blk_a", "n_std_at", "n_blk_at" (interleaved blocks and all
+ * blocks, long rows included, of the scaled A and A^T), "staged_fills" (pinned staging-ring slots filled while this
+ * session uploaded its arrays; 0 when every array took the plain copy.  The ring is shared by the device: sessions built
+ * at the same time on the same device count each other's fills too), "device_cache_hits" (device allocations served
+ * from the block cache so far in this process, by any session);
  * vectors "x", "y", "aty", "x_next", "y_next", "aty_next", "x_bar", "sum_x", "sum_y", "x_avg", "y_avg",
  * "row_scaling", "col_scaling", "scaled_values", "scaled_values_t", "scaled_c", "scaled_l", "scaled_u",
  * "scaled_lc", "scaled_uc", "x_last_restart", "y_last_restart" (scaled space unless noted). */

@@ -164,11 +164,11 @@ def column_blocks(cols, nnz, nbytes):
 # ------------------------------------------------------------------------- numpy model of the block cut (DESIGN.md section 4)
 def cut_blocks(offsets):
     """Whole consecutive rows, at most 256 entries and 256 rows per block; a longer row is a long-row block.
-    -> (interleaved blocks [(first row, one past last row)], long rows).  (Cuts never cross a 65536-row segment; the zoo
-    stays below that.)"""
+    -> (interleaved blocks [(first row, one past last row)], long rows).  (Cuts never cross a 65536-row segment: this is
+    the cut of one segment; test_wide_shapes.py models several.)"""
     off = np.asarray(offsets, np.int64)
     rows = len(off) - 1
-    assert rows < 65536
+    assert rows <= 65536
     std, long_rows, r = [], [], 0
     while r < rows:
         if off[r + 1] - off[r] > SLOTS:

@@ -33,18 +33,13 @@ def device_formulation(As, cs, ls, us, lcs, ucs, tau, sigma, px, py, radius):
     w = np.concatenate([np.full(n, 1.0 / tau), np.full(m, 1.0 / sigma)])
     lagrangian = px @ cs - px @ aty + py @ sub
     N = n + m
-    dirv, thr = np.zeros(N), np.zeros(N)
-    for k in range(N):
-        if center[k] >= up[k] and obj[k] <= 0:
-            continue
-        if center[k] <= lo[k] and obj[k] >= 0:
-            continue
-        if obj[k] == 0:
-            thr[k] = np.inf
-            continue
-        dirv[k] = -obj[k] / w[k]
-        with np.errstate(divide="ignore", invalid="ignore"):
-            thr[k] = (up[k] - center[k]) / dirv[k] if dirv[k] > 0 else (lo[k] - center[k]) / dirv[k]
+    # a component on a bound pressing outwards stays (direction 0, threshold 0); a zero gradient never stops (threshold inf)
+    stay = ((center >= up) & (obj <= 0)) | ((center <= lo) & (obj >= 0))
+    moves = ~stay & (obj != 0)
+    dirv = np.where(moves, -obj / w, 0.0)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        thr = np.where(moves, np.where(dirv > 0, (up - center) / dirv, (lo - center) / dirv),
+                       np.where(stay, 0.0, np.inf))
     tr = center.copy()
     if not (radius == 0.0 or np.sqrt(obj @ obj) == 0.0):
         high_r2 = float(np.sum(np.where(np.isinf(thr), dirv * dirv * w, 0.0)))
