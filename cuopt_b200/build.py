@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libcuopt.so")
 
-CU_SOURCES = ["pdlp_solver.cu", "csr_transpose.cu"]
+CU_SOURCES = ["pdlp_solver.cu", "csr_transpose.cu", "presolve.cu"]
 CPP_SOURCES = ["c_api.cpp", "mps_reader.cpp", "solver_settings.cpp", "dist_comm.cpp", "file_writers.cpp"]
 
 

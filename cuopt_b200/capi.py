@@ -42,6 +42,14 @@ class LPStats(C.Structure):
                 ("final_step_size", C.c_double), ("final_primal_weight", C.c_double), ("kernel_launches", C.c_int64)]
 
 
+class PresolveStats(C.Structure):
+    _fields_ = [("ran", C.c_int32), ("original_m", C.c_int32), ("original_n", C.c_int32), ("original_nnz", C.c_int32),
+                ("reduced_m", C.c_int32), ("reduced_n", C.c_int32), ("reduced_nnz", C.c_int32),
+                ("fixed_columns", C.c_int32), ("empty_rows", C.c_int32), ("singleton_rows", C.c_int32),
+                ("empty_columns", C.c_int32), ("rounds", C.c_int32), ("presolve_seconds", C.c_double),
+                ("postsolve_seconds", C.c_double)]
+
+
 class KernelProfile(C.Structure):
     _fields_ = [("ms_primal_step", C.c_double), ("ms_dual_step", C.c_double), ("ms_transpose_step", C.c_double),
                 ("bytes_primal_step", C.c_double), ("bytes_dual_step", C.c_double),
@@ -72,6 +80,7 @@ EXTENSION_SYMBOLS = [
     "cuOptB200DistInit", "cuOptB200DistDestroy", "cuOptB200SolveDistributed",
     "cuOptB200SetWarmStartCapture", "cuOptB200GetWarmStart", "cuOptB200SetWarmStart", "cuOptB200CreateWarmStart",
     "cuOptB200DestroyWarmStart", "cuOptB200WarmStartGetScalar", "cuOptB200WarmStartGetVector",
+    "cuOptB200GetPresolveStats",
 ]
 WARM_VECTORS = ("current_primal_solution", "current_dual_solution", "initial_primal_average", "initial_dual_average",
                 "current_ATY", "sum_primal_solutions", "sum_dual_solutions", "last_restart_duality_gap_primal_solution",
@@ -142,6 +151,7 @@ def lib():
                      "cuOptGetSolutionBound", "cuOptGetDualSolution", "cuOptGetReducedCosts"):
             getattr(L, name).argtypes = [vp, c_dbl_p]
         L.cuOptB200GetLPStats.argtypes = [vp, C.POINTER(LPStats)]
+        L.cuOptB200GetPresolveStats.argtypes = [vp, C.POINTER(PresolveStats)]
         L.cuOptB200SolverCreate.argtypes = [vp, vp, C.POINTER(vp)]
         L.cuOptB200SolverDestroy.argtypes = [C.POINTER(vp)]
         L.cuOptB200SolverDestroy.restype = None
@@ -400,6 +410,11 @@ class Solution:
     def stats(self) -> LPStats:
         s = LPStats()
         _check(lib().cuOptB200GetLPStats(self.h, C.byref(s)))
+        return s
+
+    def presolve_stats(self) -> PresolveStats:
+        s = PresolveStats()
+        _check(lib().cuOptB200GetPresolveStats(self.h, C.byref(s)))
         return s
 
     def warm_start(self) -> "WarmStart":

@@ -121,6 +121,12 @@ void log_solution(const pdlp_settings_t& st, const lp_problem_t& p, const lp_sol
     if (s.stats.method_stand_in == 2)
       std::fprintf(f, "method DualSimplex: this build has no CPU simplex; PDLP stands in with strict infeasibility detection "
                       "and tolerances tightened to <= 1e-8\n");
+    if (s.presolve.ran)
+      std::fprintf(f, "Presolve: %d rows, %d columns, %d nonzeros remain of %d, %d, %d (%d fixed columns, %d empty rows, "
+                      "%d singleton rows, %d empty columns; %d rounds, %.3f ms)\n", s.presolve.reduced_m, s.presolve.reduced_n,
+                   s.presolve.reduced_nnz, s.presolve.original_m, s.presolve.original_n, s.presolve.original_nnz,
+                   s.presolve.fixed_columns, s.presolve.empty_rows, s.presolve.singleton_rows, s.presolve.empty_columns,
+                   s.presolve.rounds, 1e3 * s.presolve.presolve_seconds);
     std::fprintf(f, "   Iter    Primal Obj.      Dual Obj.    Gap        Primal Res.  Dual Res.   Time\n");
     std::fprintf(f, "%7d %+.8e %+.8e  %8.2e   %8.2e     %8.2e   %.3fs\n", s.stats.number_of_steps_taken,
                  s.stats.primal_objective, s.stats.dual_objective, s.stats.gap, s.stats.l2_primal_residual,
@@ -601,6 +607,28 @@ cuopt_int_t cuOptB200GetLPStats(cuOptSolution solution, cuOptB200LPStats* stats)
   return CUOPT_SUCCESS;
 }
 
+cuopt_int_t cuOptB200GetPresolveStats(cuOptSolution solution, cuOptB200PresolveStats* stats)
+{
+  SOLUTION_OR_FAIL(stats);
+  const presolve_stats_t& t = s.sol.presolve;
+  std::memset(stats, 0, sizeof(*stats));
+  stats->ran               = t.ran;
+  stats->original_m        = t.original_m;
+  stats->original_n        = t.original_n;
+  stats->original_nnz      = t.original_nnz;
+  stats->reduced_m         = t.reduced_m;
+  stats->reduced_n         = t.reduced_n;
+  stats->reduced_nnz       = t.reduced_nnz;
+  stats->fixed_columns     = t.fixed_columns;
+  stats->empty_rows        = t.empty_rows;
+  stats->singleton_rows    = t.singleton_rows;
+  stats->empty_columns     = t.empty_columns;
+  stats->rounds            = t.rounds;
+  stats->presolve_seconds  = t.presolve_seconds;
+  stats->postsolve_seconds = t.postsolve_seconds;
+  return CUOPT_SUCCESS;
+}
+
 // ---- warm start (cuopt_b200_ext.h) ----
 namespace {
 struct warm_start_handle_t {
@@ -858,6 +886,11 @@ cuopt_int_t cuOptB200SolveDistributed(cuOptOptimizationProblem local_rows_proble
   std::unique_ptr<solution_handle_t> h(new (std::nothrow) solution_handle_t());
   if (!h) return CUOPT_OUT_OF_MEMORY;
   guarded(h->sol, [&]() {
+    if (ss.pdlp().presolve) {  // each rank holds a block of rows; presolve needs the whole matrix (checked before `dist` is used)
+      h->sol.error_status  = CUOPT_VALIDATION_ERROR;
+      h->sol.error_message = "presolve is not available in multi-GPU solves: it needs the whole matrix";
+      return;
+    }
     if (p.is_mip()) {
       h->sol.error_status  = CUOPT_VALIDATION_ERROR;
       h->sol.error_message = "cuopt-b200 implements the LP (PDLP) path only; the problem declares integer variables";

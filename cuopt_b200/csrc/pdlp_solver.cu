@@ -16,6 +16,7 @@
 
 #include "dist_comm.hpp"
 #include "pdlp_kernels.cuh"
+#include "presolve.cuh"
 #include "trust_region.cuh"
 
 #include <math_constants.h>
@@ -456,6 +457,10 @@ struct pdlp_solver_t::impl_t {
   double l2_norm_b = 0.0, l2_norm_c = 0.0;
   lp_solution_t sol;
   bool finished   = false;
+  // settings.presolve: the solver runs on the reduced problem; ps maps its solution back (postsolve_solution)
+  bool presolved    = false;
+  bool postsolved   = false;
+  presolve_state_t ps;
   double t_start  = 0.0;
   long long launches = 0;
 
@@ -536,7 +541,15 @@ struct pdlp_solver_t::impl_t {
     n        = p.n_variables;
     nnz      = p.nnz();
     maximize = p.maximize;
-    if (m == 0 || nnz == 0) {
+    if (st.presolve) {  // refused before any device work
+      if (dist != nullptr)
+        throw lp_error(error_type_t::ValidationError, "presolve is not available in multi-GPU solves: it needs the whole matrix");
+      if (st.warm_start)
+        throw lp_error(error_type_t::ValidationError, "presolve cannot be combined with a warm start");
+      if (st.capture_warm_start)
+        throw lp_error(error_type_t::ValidationError, "presolve cannot be combined with warm-start capture");
+    }
+    if (!st.presolve && (m == 0 || nnz == 0)) {
       // solve.cu:355-360: PDLP cannot run without constraints -> NumericalError solution
       throw lp_error(error_type_t::Success, "No constraints in the problem: PDLP can't be run");
     }
@@ -564,50 +577,87 @@ struct pdlp_solver_t::impl_t {
     trace.stream = stream;
     trace.mark("stream + pinned control buffers");
     const long long fills0 = staged_uploader_t::get().fills();
-    upload_csr(A, m, n, p.A_offsets, p.A_indices, p.A_values, stream, sms);
-    trace.mark("upload A + BICSR(A)");
-    transpose_to(AT, A, stream, sms);
-    trace.mark("transpose + BICSR(A^T)");
-    As.alias_structure_copy_values(A, stream);
-    ATs.alias_structure_copy_values(AT, stream);
-    const int gn = ew_grid(n, sms), gm = ew_grid(m, sms);
-    upload_staged(c, p.objective_coefficients, stream);
-    if (maximize) k_scale_constant<<<gn, EW_THREADS, 0, stream>>>(n, c.data(), -1.0);
-    if (p.variable_lower_bounds.empty()) {
-      l.resize(n);
-      k_fill<<<gn, EW_THREADS, 0, stream>>>(n, l.data(), 0.0);
-    } else {
-      upload_staged(l, p.variable_lower_bounds, stream);
-    }
-    if (p.variable_upper_bounds.empty()) {
-      u.resize(n);
-      k_fill<<<gn, EW_THREADS, 0, stream>>>(n, u.data(), std::numeric_limits<double>::infinity());
-    } else {
-      upload_staged(u, p.variable_upper_bounds, stream);
-    }
-    if (!p.constraint_lower_bounds.empty()) {
-      upload_staged(lc, p.constraint_lower_bounds, stream);
-      upload_staged(uc, p.constraint_upper_bounds, stream);
-    } else {
-      hvec<double> hlc, huc;
-      p.row_bounds(hlc, huc);
-      upload_staged(lc, hlc, stream);
-      upload_staged(uc, huc, stream);
-      sync();  // hlc / huc go out of scope
-    }
-    {
-      dvec<int> bad(2);
-      bad.zero(stream);
-      k_count_crossed_bounds<<<gn, EW_THREADS, 0, stream>>>(n, l.data(), u.data(), bad.data());
-      k_count_crossed_bounds<<<gm, EW_THREADS, 0, stream>>>(m, lc.data(), uc.data(), bad.data() + 1);
-      check_launch();
-      int h_bad[2] = {0, 0};
-      CUOPT_CUDA_TRY(cudaMemcpyAsync(h_bad, bad.data(), sizeof(h_bad), cudaMemcpyDeviceToHost, stream));
+    auto upload_vectors = [&]() {  // c (negated when maximising), bounds with their defaults, the crossed-bound checks
+      const int gn = ew_grid(n, sms), gm = ew_grid(m, sms);
+      upload_staged(c, p.objective_coefficients, stream);
+      if (maximize) k_scale_constant<<<gn, EW_THREADS, 0, stream>>>(n, c.data(), -1.0);
+      if (p.variable_lower_bounds.empty()) {
+        l.resize(n);
+        k_fill<<<gn, EW_THREADS, 0, stream>>>(n, l.data(), 0.0);
+      } else {
+        upload_staged(l, p.variable_lower_bounds, stream);
+      }
+      if (p.variable_upper_bounds.empty()) {
+        u.resize(n);
+        k_fill<<<gn, EW_THREADS, 0, stream>>>(n, u.data(), std::numeric_limits<double>::infinity());
+      } else {
+        upload_staged(u, p.variable_upper_bounds, stream);
+      }
+      if (!p.constraint_lower_bounds.empty()) {
+        upload_staged(lc, p.constraint_lower_bounds, stream);
+        upload_staged(uc, p.constraint_upper_bounds, stream);
+      } else {
+        hvec<double> hlc, huc;
+        p.row_bounds(hlc, huc);
+        upload_staged(lc, hlc, stream);
+        upload_staged(uc, huc, stream);
+        sync();  // hlc / huc go out of scope
+      }
+      {
+        dvec<int> bad(2);
+        bad.zero(stream);
+        k_count_crossed_bounds<<<gn, EW_THREADS, 0, stream>>>(n, l.data(), u.data(), bad.data());
+        k_count_crossed_bounds<<<gm, EW_THREADS, 0, stream>>>(m, lc.data(), uc.data(), bad.data() + 1);
+        check_launch();
+        int h_bad[2] = {0, 0};
+        CUOPT_CUDA_TRY(cudaMemcpyAsync(h_bad, bad.data(), sizeof(h_bad), cudaMemcpyDeviceToHost, stream));
+        sync();
+        if (h_bad[0]) throw lp_error(error_type_t::ValidationError, "Variable lower bound above upper bound");
+        if (h_bad[1]) throw lp_error(error_type_t::ValidationError, "Constraint lower bound above upper bound");
+      }
+    };
+    if (st.presolve) {
+      // plain CSR and vectors, presolve (presolve.cu), then the reduced matrix takes the path of an unpresolved one
+      A.rows = m;
+      A.cols = n;
+      A.nnz  = nnz;
+      upload_staged(A.off, p.A_offsets, stream);
+      upload_staged(A.idx, p.A_indices, stream);
+      upload_staged(A.val, p.A_values, stream);
+      upload_vectors();
+      trace.mark("upload A + objective / bound vectors");
+      presolve_device(m, n, A.off, A.idx, A.val, c, l, u, lc, uc, st.absolute_primal_tolerance, ps, stream, trace.on);
+      presolved = true;
+      nnz       = ps.nnz1;
+      trace.mark("presolve");
+      staged_fills = staged_uploader_t::get().fills() - fills0;
+      if (ps.verdict != termination_status_t::NoTermination) {
+        finish_in_presolve();
+        return;
+      }
+      obj_offset += obj_scale * ps.offset;
+      A.rows = m;
+      A.cols = n;
+      A.nnz  = nnz;
+      std::vector<int> hoff((size_t)m + 1);
+      A.off.download(hoff.data(), stream);
       sync();
-      if (h_bad[0]) throw lp_error(error_type_t::ValidationError, "Variable lower bound above upper bound");
-      if (h_bad[1]) throw lp_error(error_type_t::ValidationError, "Constraint lower bound above upper bound");
+      build_bicsr(A, hoff, stream, sms);
+      trace.mark("BICSR(reduced A)");
+      transpose_to(AT, A, stream, sms);
+      trace.mark("transpose + BICSR(A^T)");
+      As.alias_structure_copy_values(A, stream);
+      ATs.alias_structure_copy_values(AT, stream);
+    } else {
+      upload_csr(A, m, n, p.A_offsets, p.A_indices, p.A_values, stream, sms);
+      trace.mark("upload A + BICSR(A)");
+      transpose_to(AT, A, stream, sms);
+      trace.mark("transpose + BICSR(A^T)");
+      As.alias_structure_copy_values(A, stream);
+      ATs.alias_structure_copy_values(AT, stream);
+      upload_vectors();
+      staged_fills = staged_uploader_t::get().fills() - fills0;
     }
-    staged_fills = staged_uploader_t::get().fills() - fills0;
     cs.copy_from(c, stream); ls.copy_from(l, stream); us.copy_from(u, stream); lcs.copy_from(lc, stream); ucs.copy_from(uc, stream);
     trace.mark("objective / bound vectors");
 
@@ -1443,6 +1493,7 @@ struct pdlp_solver_t::impl_t {
 
   void fetch_ctl()
   {
+    if (d_ctl.size() == 0) return;  // presolve decided the problem: no PDLP state was built
     CUOPT_CUDA_TRY(cudaMemcpyAsync(h_ctl, d_ctl.data(), sizeof(pdhg_ctl_t), cudaMemcpyDeviceToHost, stream));
     sync();
   }
@@ -1583,6 +1634,56 @@ struct pdlp_solver_t::impl_t {
     check_launch();
     CUOPT_CUDA_TRY(cudaMemcpyAsync(h_eval, d_eval.data(), 2 * sizeof(eval_t), cudaMemcpyDeviceToHost, stream));
     sync();
+  }
+
+  // ---- presolve (presolve.cu) ----
+  // The problem was decided in presolve: no PDLP state is built.  Optimal: every column has its value and the duals come from
+  // postsolve; infeasible or unbounded: zero vectors of the original sizes (presolve has no certificate).
+  void finish_in_presolve()
+  {
+    sol.termination_status   = ps.verdict;
+    sol.error_status         = 0;
+    sol.stats.solved_by_pdlp = 0;
+    if (ps.verdict == termination_status_t::Optimal) {
+      const double t0 = now_seconds();
+      postsolve_device(ps, {}, {}, {}, false, sol.primal, sol.dual, sol.reduced_cost, stream);
+      ps.stats.postsolve_seconds = now_seconds() - t0;
+      const double obj           = obj_scale * ps.offset + obj_offset;
+      sol.stats.primal_objective = obj;
+      sol.stats.dual_objective   = obj;
+    } else {
+      sol.primal.assign(ps.n0, 0.0);
+      sol.dual.assign(ps.m0, 0.0);
+      sol.reduced_cost.assign(ps.n0, 0.0);
+    }
+    sol.presolve = ps.stats;
+    initialised = finished = postsolved = true;
+  }
+  // Every ending of a presolved solve: the reduced-space vectors fill_solution / fill_best_solution left in sol go back to
+  // the original sizes.  Infeasibility verdicts carry certificates: scattered, zeros elsewhere.  When presolve removed nothing
+  // the vectors are already those of the original problem.  An ending without vectors (NumericalError) keeps none.
+  void postsolve_solution()
+  {
+    if (!presolved || postsolved) return;
+    postsolved = true;
+    nvtx_range_t nvtx_scope("postsolve");
+    const bool certificate = sol.termination_status == termination_status_t::PrimalInfeasible ||
+                             sol.termination_status == termination_status_t::DualInfeasible;
+    if (!ps.removed_nothing() && !(sol.primal.empty() && sol.dual.empty())) {
+      CUOPT_CUDA_TRY(cudaEventRecord(ev_a, stream));
+      std::vector<double> x, y, r;
+      postsolve_device(ps, sol.primal, sol.dual, sol.reduced_cost, certificate, x, y, r, stream);
+      CUOPT_CUDA_TRY(cudaEventRecord(ev_b, stream));
+      CUOPT_CUDA_TRY(cudaEventSynchronize(ev_b));
+      float ms = 0.f;
+      cudaEventElapsedTime(&ms, ev_a, ev_b);
+      ps.stats.postsolve_seconds = 1e-3 * ms;
+      sol.primal       = std::move(x);
+      sol.dual         = std::move(y);
+      sol.reduced_cost = std::move(r);
+    }
+    sol.presolve = ps.stats;
+    trace.mark("postsolve");
   }
 
   void fill_solution(bool average, termination_status_t status)  // termination_strategy.cu:270-357
@@ -1959,7 +2060,10 @@ struct pdlp_solver_t::impl_t {
         CUOPT_CUDA_TRY(cudaEventRecord(ev_a, stream));
         sol.stats.n_major_iterations += 1;
         evaluate_iterates();
-        if (check_termination()) return true;
+        if (check_termination()) {
+          postsolve_solution();
+          return true;
+        }
         const int cur = h_ctl->parity;
         if (hp.rescale_for_restart) {  // pdlp.cu:1144-1149
           k_scale_back<<<grid_n, EW_THREADS, 0, stream>>>(n, x_avg.data(), Dc.data());
@@ -2067,6 +2171,7 @@ double pdlp_solver_t::scalar(const std::string& name)
   if (name == "n_blk_at") return s.ATs.bi_structure().n_blk;
   if (name == "staged_fills") return (double)s.staged_fills;
   if (name == "device_cache_hits") return (double)device_block_cache_t::get().hits();
+  if (name == "presolve_offset") return s.ps.offset;
   return std::nan("");
 }
 
@@ -2098,6 +2203,21 @@ std::vector<double> pdlp_solver_t::vector(const std::string& name)
   else if (name == "scaled_uc") v = &s.ucs;
   else if (name == "x_last_restart") v = &s.x_lr;
   else if (name == "y_last_restart") v = &s.y_lr;
+  if (name.rfind("presolve_", 0) == 0) {  // the reduced problem (unscaled, minimisation form) and its maps
+    if (!s.presolved) throw lp_error(error_type_t::InvalidArgument, name + ": the session was not presolved");
+    const dvec<int>* map = name == "presolve_row_map" ? &s.ps.row_map : name == "presolve_col_map" ? &s.ps.col_map : nullptr;
+    if (map) {
+      std::vector<int> hi(map->size());
+      map->download(hi.data(), s.stream);
+      s.sync();
+      return std::vector<double>(hi.begin(), hi.end());
+    }
+    if (name == "presolve_c") v = &s.c;
+    else if (name == "presolve_l") v = &s.l;
+    else if (name == "presolve_u") v = &s.u;
+    else if (name == "presolve_lc") v = &s.lc;
+    else if (name == "presolve_uc") v = &s.uc;
+  }
   if (!v) throw lp_error(error_type_t::InvalidArgument, "unknown vector " + name);
   std::vector<double> h(v->size());
   v->download(h.data(), s.stream);

@@ -186,6 +186,7 @@ struct pdlp_settings_t {
   // extension (cuopt_b200_ext.h): continue from a previous solve / make the solution carry the state to do so
   std::shared_ptr<const pdlp_warm_start_t> warm_start;
   bool capture_warm_start = false;
+  bool presolve           = false;  // extension: presolve.cu before PDLP, postsolve after
 };
 
 // additional_termination_information_t (pdlp/solver_solution.hpp:47-87) plus timing of this build.
@@ -216,6 +217,16 @@ struct lp_stats_t {
   double final_primal_weight = 0;
 };
 
+// What presolve removed and what it and postsolve cost (cuOptB200PresolveStats).
+struct presolve_stats_t {
+  int ran = 0;  // 1 when the solve was presolved
+  int original_m = 0, original_n = 0, original_nnz = 0;
+  int reduced_m = 0, reduced_n = 0, reduced_nnz = 0;
+  int fixed_columns = 0, empty_rows = 0, singleton_rows = 0, empty_columns = 0;
+  int rounds = 0;
+  double presolve_seconds = 0, postsolve_seconds = 0;  // device time (CUDA events)
+};
+
 struct lp_solution_t {
   termination_status_t termination_status = termination_status_t::NoTermination;
   int error_status                        = 0;  // error_type_t
@@ -223,6 +234,7 @@ struct lp_solution_t {
   std::vector<double> primal, dual, reduced_cost;
   lp_stats_t stats;
   std::shared_ptr<pdlp_warm_start_t> warm_start;  // filled when settings.capture_warm_start
+  presolve_stats_t presolve;
 };
 
 }  // namespace cuopt_b200

@@ -1,6 +1,7 @@
 #include "solver_settings.hpp"
 
 #include <cuopt/linear_programming/constants.h>
+#include <cuopt_b200/cuopt_b200_ext.h>
 
 #include <limits>
 
@@ -57,6 +58,7 @@ solver_settings_t::solver_settings_t()
     {CUOPT_LOG_TO_CONSOLE, &pdlp_.log_to_console, false, true},
     {CUOPT_LOG_TO_CONSOLE, &mip_log_to_console_, false, true},
     {CUOPT_CROSSOVER, &pdlp_.crossover, false, true},
+    {CUOPT_B200_PRESOLVE, &pdlp_.presolve, false, true},
   };
   strings_ = {
     {CUOPT_LOG_FILE, &mip_log_file_, "", ""},

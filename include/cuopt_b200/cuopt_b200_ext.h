@@ -49,6 +49,27 @@ typedef struct cuOptB200LPStats {
 /* Statistics of an LP solution returned by cuOptSolve. */
 cuopt_int_t cuOptB200GetLPStats(cuOptSolution solution, cuOptB200LPStats* stats);
 
+/* ---- presolve --------------------------------------------------------------------------------------------------
+ * Bool parameter (cuOptSetIntegerParameter / cuOptSetParameter / cuopt_cli --presolve true), default false.  When on, the
+ * solver first removes, in rounds on the device, fixed columns, empty rows, singleton rows (turned into column bounds) and
+ * empty columns, runs PDLP on what is left and maps the solution back to the original rows and columns (postsolve of
+ * primal, dual and reduced costs).  Reported objectives include the removed columns; residuals are those of the reduced
+ * problem.  Refused with CUOPT_VALIDATION_ERROR together with a warm start, warm-start capture or
+ * cuOptB200SolveDistributed.  INTEGRATION.md "presolve". */
+#define CUOPT_B200_PRESOLVE "presolve"
+
+typedef struct cuOptB200PresolveStats {
+  cuopt_int_t ran; /* 1 when the solve was presolved */
+  cuopt_int_t original_m, original_n, original_nnz;
+  cuopt_int_t reduced_m, reduced_n, reduced_nnz; /* stored zeros are dropped from the reduced matrix */
+  cuopt_int_t fixed_columns, empty_rows, singleton_rows, empty_columns; /* removed by each rule */
+  cuopt_int_t rounds;
+  cuopt_float_t presolve_seconds, postsolve_seconds; /* device time */
+} cuOptB200PresolveStats;
+
+/* Presolve statistics of a solution (all zero when presolve was off). */
+cuopt_int_t cuOptB200GetPresolveStats(cuOptSolution solution, cuOptB200PresolveStats* stats);
+
 /* ---- solver session: the same solver cuOptSolve runs, driven step by step -------------------- */
 typedef void* cuOptB200Solver;
 
@@ -88,7 +109,11 @@ cuopt_int_t cuOptB200SolverAdvance(cuOptB200Solver solver, cuopt_int_t accepted_
  * from the block cache so far in this process, by any session);
  * vectors "x", "y", "aty", "x_next", "y_next", "aty_next", "x_bar", "sum_x", "sum_y", "x_avg", "y_avg",
  * "row_scaling", "col_scaling", "scaled_values", "scaled_values_t", "scaled_c", "scaled_l", "scaled_u",
- * "scaled_lc", "scaled_uc", "x_last_restart", "y_last_restart" (scaled space unless noted). */
+ * "scaled_lc", "scaled_uc", "x_last_restart", "y_last_restart" (scaled space unless noted).
+ * Presolved sessions: the vectors above are of the reduced problem; "presolve_row_map", "presolve_col_map" (original
+ * index of each kept row / column), "presolve_c", "presolve_l", "presolve_u", "presolve_lc", "presolve_uc" (the reduced
+ * problem, unscaled, in minimisation form: c negated when maximising) and the scalar "presolve_offset" (objective of the
+ * removed columns, same form).  cuOptB200SolverGetSolution returns the postsolved solution. */
 cuopt_int_t cuOptB200SolverGetScalar(cuOptB200Solver solver, const char* name, cuopt_float_t* value_ptr);
 cuopt_int_t cuOptB200SolverGetVector(cuOptB200Solver solver,
                                      const char* name,
