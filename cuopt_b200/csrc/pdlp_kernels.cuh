@@ -248,7 +248,8 @@ __global__ void __launch_bounds__(EW_THREADS) k_primal_step(const pdhg_ctl_t* __
 // INIT: the product continues the running sum t of the earlier column blocks (gather blocking: this is the LAST block's pass)
 // BCAST (multi-GPU "gather" transport): y' of this rank's rows also goes to the packed y' buffer of every rank that reads
 // the row (peer stores over NVLink, y_peers.p[r] = rank r's buffer) and the last CTA raises the y' flag.
-template <bool INIT, int NPRE, bool BCAST = false>
+// FMT: storage form of A (spmv_bicsr.cuh BICSR_FMT_*)
+template <bool INIT, int NPRE, bool BCAST = false, int FMT = 0>
 __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_dual_step(pdhg_ctl_t* __restrict__ ctl,
                                                                              bicsr_view_t A,
                                                                              const double* __restrict__ xbar,
@@ -312,7 +313,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_dual_st
     const double d   = next - p.y;
     dy2 += d * d;
   };
-  spmv_bicsr_rows<payload_t, INIT, NPRE>(A, xbar, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
+  spmv_bicsr_rows<payload_t, INIT, NPRE, FMT>(A, xbar, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
   const double tot = block_reduce(dy2, red);
   if (threadIdx.x == 0) part_dy2[blockIdx.x] = tot;
   if constexpr (BCAST) peer_signal_grid_done(&ctl->ticket[2], flags, world, DIST_FLAG_Y + rank, epoch, DIST_FLAG_Y_B + rank);
@@ -324,7 +325,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_dual_st
 // interaction = dx . (A^T y' - A^T y)  (the reference's SpMV-saving form, :267-277).
 // =============================================================================================
 // INIT: as in k_dual_step (the last column block's pass of a gather-blocked A^T y')
-template <bool INIT, int NPRE>
+template <bool INIT, int NPRE, int FMT = 0>
 __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_transpose_step(pdhg_ctl_t* __restrict__ ctl,
                                                                                   bicsr_view_t AT,
                                                                                   const double* __restrict__ ybuf0,
@@ -364,7 +365,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, bicsr_min_ctas(NPRE)) k_transpo
     acc[0] += p.dx * (s - p.aty);
     acc[1] += p.dx * p.dx;
   };
-  spmv_bicsr_rows<payload_t, INIT, NPRE>(AT, yn, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
+  spmv_bicsr_rows<payload_t, INIT, NPRE, FMT>(AT, yn, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
 
   if (!publish_and_elect<2>(acc, parts, &ctl->ticket[0], red)) return;
   const double interaction = gather_partials(parts, gridDim.x, red);
@@ -795,6 +796,7 @@ __global__ void k_step_rule_gather(pdhg_ctl_t* __restrict__ ctl, const double* _
 // t[r] = (first ? 0 : t[r]) + sum over the entries of row r in this column block.
 //   pick_candidate = 0: x = x0;  1: x = the candidate dual y' = parity ? x0 : x1  (K3).
 //   wait_flags: gather transport only, first pass of K2 / K3 (the other ranks' xbar / y' entries must have landed).
+template <int FMT = 0>
 __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_block_pass(const pdhg_ctl_t* __restrict__ ctl,
                                                                               bicsr_view_t Ab,
                                                                               const double* __restrict__ x0,
@@ -819,7 +821,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_block_pass(co
     return p;
   };
   auto row_op = [&](int r, double s, const payload_t&) { st_l2(t + r, s, pol.stream); };
-  spmv_bicsr_rows<payload_t, true>(Ab, x, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
+  spmv_bicsr_rows<payload_t, true, 1, FMT>(Ab, x, rows[threadIdx.x >> 5], pre_op, row_op, pol.keep);
 }
 
 // Applies a still-pending running-average update (end of a batch, before averages are formed).
@@ -868,6 +870,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_spmv(bicsr_vi
 //   out_u = M u, out_v = M v  (first),   out_u += M u, out_v += M v  (otherwise).
 // A gather-blocked matrix runs one launch per column block, in block order (first = block 0): the sums of a row come out in
 // the order of k_block_pass.  An unblocked matrix is one first pass, whose sums are exactly k_spmv's.
+template <int FMT = 0>
 __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_spmv_pair(bicsr_view_t M,
                                                                              const double* __restrict__ u,
                                                                              const double* __restrict__ v,
@@ -881,7 +884,7 @@ __global__ void __launch_bounds__(BICSR_THREADS, BICSR_MIN_CTAS) k_spmv_pair(bic
     out_v[r] = first ? sv : out_v[r] + sv;
   };
   const int w = threadIdx.x >> 5;
-  spmv_bicsr_rows_pair(M, u, v, rows[0][w], rows[1][w], row_op, make_l2_policies(g_l2_hints).keep);
+  spmv_bicsr_rows_pair<FMT>(M, u, v, rows[0][w], rows[1][w], row_op, make_l2_policies(g_l2_hints).keep);
 }
 
 // =============================================================================================

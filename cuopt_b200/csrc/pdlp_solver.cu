@@ -40,10 +40,14 @@ namespace {
 // Block-interleaved storage of a matrix (spmv_bicsr.cuh): what every SpMV kernel reads.
 struct bicsr_dev_t {
   int n_std = 0, n_blk = 0;
+  int fmt = 0, col0 = 0;  // storage form (BICSR_FMT_* bits): compact forms hold lo16 / hi8 instead of idx, mask instead of row_slot
   dvec<int2> desc;
   dvec<unsigned short> row_slot;
   dvec<int> idx;
   dvec<double> val;
+  dvec<unsigned short> lo16;
+  dvec<unsigned long long> hi8;
+  dvec<unsigned> mask;
 };
 
 // A matrix on the device: plain CSR (setup kernels: scaling statistics, transpose, column split; long rows of the SpMV)
@@ -61,8 +65,8 @@ struct csr_dev_t {
   bicsr_view_t view() const
   {
     const bicsr_dev_t& s = bi_structure();
-    return bicsr_view_t{s.desc.data(), s.row_slot.data(), s.idx.data(), bi.val.data(), s.n_std, s.n_blk,
-                        off_ptr(),     idx_ptr(),         val.data()};
+    return bicsr_view_t{s.desc.data(), s.row_slot.data(), s.idx.data(), bi.val.data(), s.n_std,  s.n_blk, off_ptr(),
+                        idx_ptr(),     val.data(),        s.lo16.data(), s.hi8.data(), s.mask.data(), s.col0};
   }
   // same sparsity pattern, own values (device-to-device copy)
   void alias_structure_copy_values(const csr_dev_t& o, cudaStream_t s)
@@ -156,6 +160,41 @@ void fill_bicsr_values(csr_dev_t& d, cudaStream_t s, int sms)
     const int grid = std::max(1, std::min((st.n_std + 7) / 8, sms * 8));
     k_bicsr_fill_values<<<grid, 256, 0, s>>>(st.n_std, st.desc.data(), d.off_ptr(), d.val.data(), d.bi.val.data());
     CUOPT_CUDA_TRY(cudaGetLastError());
+  }
+}
+
+// Rewrites the structure of d (built by build_bicsr) in the compact form fmt (spmv_bicsr.cuh): three-byte indices relative
+// to col0 and / or the non-empty-row mask; the arrays the form no longer reads are freed.
+void compact_bicsr(csr_dev_t& d, int fmt, int col0, cudaStream_t s, int sms)
+{
+  bicsr_dev_t& b = d.bi;
+  b.fmt  = fmt;
+  b.col0 = col0;
+  if (fmt == 0 || b.n_std == 0) return;
+  const size_t ns = (size_t)b.n_std;
+  if (fmt & BICSR_FMT_IDX3) {
+    b.lo16.resize(ns * BICSR_SLOTS);
+    b.hi8.resize(ns * 32);
+  }
+  if (fmt & BICSR_FMT_MASK) b.mask.resize(ns * 8);
+  const int grid = std::max(1, std::min((b.n_std + BICSR_WARPS - 1) / BICSR_WARPS, sms * 8));
+  k_bicsr_fill_structure<<<grid, BICSR_THREADS, 0, s>>>(b.n_std, b.desc.data(), d.off.data(), d.idx.data(), col0,
+                                                        b.lo16.data(), b.hi8.data(), b.mask.data());
+  CUOPT_CUDA_TRY(cudaGetLastError());
+  CUOPT_CUDA_TRY(cudaStreamSynchronize(s));
+  if (fmt & BICSR_FMT_IDX3) b.idx = dvec<int>{};
+  if (fmt & BICSR_FMT_MASK) b.row_slot = dvec<unsigned short>{};
+}
+
+// Calls f(std::integral_constant<int, fmt>) for a storage form known at run time.
+template <typename F>
+void with_fmt(int fmt, F&& f)
+{
+  switch (fmt) {
+    case BICSR_FMT_IDX3: f(std::integral_constant<int, BICSR_FMT_IDX3>{}); break;
+    case BICSR_FMT_MASK: f(std::integral_constant<int, BICSR_FMT_MASK>{}); break;
+    case BICSR_FMT_IDX3 | BICSR_FMT_MASK: f(std::integral_constant<int, BICSR_FMT_IDX3 | BICSR_FMT_MASK>{}); break;
+    default: f(std::integral_constant<int, 0>{});
   }
 }
 
@@ -415,6 +454,9 @@ struct pdlp_solver_t::impl_t {
   int occ_spmv = 1;   // resident CTAs per SM of the SpMV kernels (64 registers, 16 KB of shared memory)
   int occ_spmv2 = 1;  // ... of the fused kernels that prefetch the payload of two row groups (85 registers)
   int npre_override = 0;  // experiment switch CUOPT_B200_SPMV_NPRE=1|2
+  // CUOPT_B200_COMPACT_BLOCKS: storage form of the column blocks of a single-GPU gather-blocked product (BICSR_FMT_* bits,
+  // default 3): 1 three-byte block-local indices, 2 non-empty-row masks; 0 = the plain form (A/B runs, tests)
+  int compact_blocks = BICSR_FMT_IDX3 | BICSR_FMT_MASK;
   dvec<double> eval_m, eval_n;  // A x (current, average) and, on one GPU, A^T y (current, average)
   dvec<double> part_max;        // per_constraint_residual: per-CTA maxima, rows (2 x grid_m) then columns (2 x grid_n)
   dvec<double> part_infeas;     // infeasibility detection: rows (6 x grid_m) then columns (12 x grid_n)
@@ -432,6 +474,7 @@ struct pdlp_solver_t::impl_t {
   // is L2-sized; B == 1 (small LPs) keeps the fused kernels
   struct gather_blocks_t {
     int B = 1, width = 0;
+    int fmt = 0;  // storage form of the blocks (and of their unscaled copies), BICSR_FMT_* bits
     std::vector<csr_dev_t> blk;
     std::vector<csr_dev_t> unscaled;  // single GPU: the same blocks with the unscaled values (termination evaluation)
     std::vector<int> grid;  // per block, for the schedule (wide or not) its pass uses
@@ -714,6 +757,7 @@ struct pdlp_solver_t::impl_t {
       gather_block_bytes = (size_t)((double)l2 * GATHER_BLOCK_L2_FRACTION);
     }
     if (const char* e = std::getenv("CUOPT_B200_GATHER_BLOCK_BYTES")) gather_block_bytes = (size_t)std::atoll(e);
+    if (const char* e = std::getenv("CUOPT_B200_COMPACT_BLOCKS")) compact_blocks = std::atoi(e) & (BICSR_FMT_IDX3 | BICSR_FMT_MASK);
     part_k3.resize(2 * (size_t)std::max({grid_k3, grid_n, sms * 16}));
     part_rows.resize(6 * (size_t)grid_m);
     if (hp.restart_strategy == 2) {
@@ -1235,6 +1279,10 @@ struct pdlp_solver_t::impl_t {
     }
     if (B <= 1) return;
     g.B = B;
+    if (forced_width == 0 && !sharded()) {  // the sharded transports keep the plain form
+      g.fmt = compact_blocks;
+      if (g.width > BICSR_IDX3_MAX_WIDTH) g.fmt &= ~BICSR_FMT_IDX3;
+    }
     g.blk.resize(B);
     std::vector<int*> offs(B), idxs(B);
     std::vector<double*> vals(B);
@@ -1261,6 +1309,7 @@ struct pdlp_solver_t::impl_t {
       g.blk[b].off.download(hoff.data(), stream);
       sync();
       build_bicsr(g.blk[b], hoff, stream, sms);
+      compact_bicsr(g.blk[b], g.fmt, b * g.width, stream, sms);
       g.grid[b] = spmv_grid(g.blk[b]);
     }
     if (unscaled_src) {  // the cut depends on the structure only, which M shares with unscaled_src
@@ -1293,8 +1342,10 @@ struct pdlp_solver_t::impl_t {
   {
     for (int b = 0; b < count; ++b) {
       const csr_dev_t& M = g.blk[b];
-      k_block_pass<<<g.grid[b], BICSR_THREADS, 0, stream>>>(d_ctl.data(), M.view(), x0, x1, pick_candidate, t, b == 0,
-                                                            b == 0 ? wait_flags : nullptr, n_wait);
+      with_fmt(g.fmt, [&](auto F) {
+        k_block_pass<decltype(F)::value><<<g.grid[b], BICSR_THREADS, 0, stream>>>(
+          d_ctl.data(), M.view(), x0, x1, pick_candidate, t, b == 0, b == 0 ? wait_flags : nullptr, n_wait);
+      });
     }
   }
   // K2: one fused kernel; with gather blocking (B - 1) payload-free passes over the first column blocks, then the fused kernel
@@ -1311,10 +1362,10 @@ struct pdlp_solver_t::impl_t {
     const double* t     = blocked ? t_m.data() : nullptr;
     const unsigned long long* wf = wait_flags_b ? wait_flags_b : (blocked ? nullptr : wait_flags);
     if (blocked) launch_block_passes(blkA, blkA.B - 1, xbar.data(), xbar.data(), 0, t_m.data(), wait_flags, n_wait);
-#define CUOPT_K2(INIT, NPRE)                                                                                             \
-  k_dual_step<INIT, NPRE><<<grid, BICSR_THREADS, 0, stream>>>(d_ctl.data(), L.view(), xbar.data(), ybuf[0].data(),       \
-                                                              ybuf[1].data(), lcs.data(), ucs.data(), sum_y.data(),      \
-                                                              part_dy2.data(), wf, n_wait, t)
+#define CUOPT_K2(INIT, NPRE, FMT)                                                                                        \
+  k_dual_step<INIT, NPRE, false, FMT><<<grid, BICSR_THREADS, 0, stream>>>(                                               \
+    d_ctl.data(), L.view(), xbar.data(), ybuf[0].data(), ybuf[1].data(), lcs.data(), ucs.data(), sum_y.data(),          \
+    part_dy2.data(), wf, n_wait, t)
 #define CUOPT_K2B(INIT, NPRE)                                                                                            \
   k_dual_step<INIT, NPRE, true><<<grid, BICSR_THREADS, 0, stream>>>(d_ctl.data(), L.view(), xbar.data(), ybuf[0].data(), \
                                                                     ybuf[1].data(), lcs.data(), ucs.data(), sum_y.data(), \
@@ -1323,8 +1374,11 @@ struct pdlp_solver_t::impl_t {
     if (bcast) {
       if (blocked) { if (npre > 1) CUOPT_K2B(true, 2); else CUOPT_K2B(true, 1); }
       else { if (npre > 1) CUOPT_K2B(false, 2); else CUOPT_K2B(false, 1); }
-    } else if (blocked) { if (npre > 1) CUOPT_K2(true, 2); else CUOPT_K2(true, 1); }
-    else { if (npre > 1) CUOPT_K2(false, 2); else CUOPT_K2(false, 1); }
+    } else if (blocked) {
+      with_fmt(blkA.fmt, [&](auto F) {
+        if (npre > 1) CUOPT_K2(true, 2, decltype(F)::value); else CUOPT_K2(true, 1, decltype(F)::value);
+      });
+    } else { if (npre > 1) CUOPT_K2(false, 2, 0); else CUOPT_K2(false, 1, 0); }
 #undef CUOPT_K2B
 #undef CUOPT_K2
   }
@@ -1344,13 +1398,15 @@ struct pdlp_solver_t::impl_t {
     const int grid     = k3_grid();
     const double* t    = blocked ? t_n.data() : nullptr;
     if (blocked) launch_block_passes(blkAT, blkAT.B - 1, ybuf[0].data(), ybuf[1].data(), 1, t_n.data(), nullptr, 0);
-#define CUOPT_K3(INIT, NPRE)                                                                                              \
-  k_transpose_step<INIT, NPRE><<<grid, BICSR_THREADS, 0, stream>>>(d_ctl.data(), L.view(), ybuf[0].data(), ybuf[1].data(), \
-                                                                   xbuf[0].data(), xbuf[1].data(), atybuf[0].data(),      \
-                                                                   atybuf[1].data(), part_k3.data(), part_dy2.data(),     \
-                                                                   n_part_dy2, t)
-    if (blocked) { if (npre > 1) CUOPT_K3(true, 2); else CUOPT_K3(true, 1); }
-    else { if (npre > 1) CUOPT_K3(false, 2); else CUOPT_K3(false, 1); }
+#define CUOPT_K3(INIT, NPRE, FMT)                                                                                         \
+  k_transpose_step<INIT, NPRE, FMT><<<grid, BICSR_THREADS, 0, stream>>>(                                                  \
+    d_ctl.data(), L.view(), ybuf[0].data(), ybuf[1].data(), xbuf[0].data(), xbuf[1].data(), atybuf[0].data(),            \
+    atybuf[1].data(), part_k3.data(), part_dy2.data(), n_part_dy2, t)
+    if (blocked) {
+      with_fmt(blkAT.fmt, [&](auto F) {
+        if (npre > 1) CUOPT_K3(true, 2, decltype(F)::value); else CUOPT_K3(true, 1, decltype(F)::value);
+      });
+    } else { if (npre > 1) CUOPT_K3(false, 2, 0); else CUOPT_K3(false, 1, 0); }
 #undef CUOPT_K3
   }
   int kernels_per_attempt() const
@@ -1384,7 +1440,9 @@ struct pdlp_solver_t::impl_t {
     const int count = g.unscaled.empty() ? 1 : (int)g.unscaled.size();
     for (int b = 0; b < count; ++b) {
       const csr_dev_t& Mb = g.unscaled.empty() ? M : g.unscaled[b];
-      k_spmv_pair<<<spmv_grid(Mb), BICSR_THREADS, 0, stream>>>(Mb.view(), u, v, out_u, out_v, b == 0);
+      with_fmt(g.fmt, [&](auto F) {  // g.fmt is 0 without unscaled blocks
+        k_spmv_pair<decltype(F)::value><<<spmv_grid(Mb), BICSR_THREADS, 0, stream>>>(Mb.view(), u, v, out_u, out_v, b == 0);
+      });
     }
     return count;
   }
@@ -2153,6 +2211,8 @@ double pdlp_solver_t::scalar(const std::string& name)
   if (name == "last_restart_was_average") return s.last_restart_was_average ? 1.0 : 0.0;
   if (name == "eval_blocks") return (double)std::max<size_t>(1, s.blkA.unscaled.size());  // passes of the evaluation's A x
   if (name == "eval_blocks_t") return (double)std::max<size_t>(1, s.blkAT.unscaled.size());
+  if (name == "blocks_form_a") return s.blkA.fmt;  // BICSR_FMT_* bits of the column blocks
+  if (name == "blocks_form_at") return s.blkAT.fmt;
   if (name == "valid") return k.valid;
   // launch geometry (read-only): grid_k2 / grid_k3 as the fused K2 / K3 launch (on the last column block when blocked),
   // n_std / n_blk of the whole scaled A and A^T

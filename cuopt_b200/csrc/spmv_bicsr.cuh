@@ -22,6 +22,16 @@
 // shared-memory wavefronts and every per-entry bank conflict from the L1TEX unit that also has to serve the gathers
 // (scripts/spmv_lab.cu compares the two).
 //
+// Compact form (column blocks of a gather-blocked product on one GPU, template parameter FMT of the kernels below).
+//   BICSR_FMT_IDX3: an entry's column is stored RELATIVE TO THE FIRST COLUMN OF ITS COLUMN BLOCK (col0; the gathers read
+//     x + col0) in three bytes: the low 16 bits in lo16, lane-major (lane l's entries 8 l .. 8 l + 7 are one 16-byte
+//     word), and one 8-byte word hi8 per lane whose byte k holds the high 5 bits of its entry k, BICSR_HI_PAD (bit 6) for an
+//     unused slot and BICSR_HI_END (bit 7) for the last entry of a row.  Needs a column block of at most 2^21 columns.
+//   BICSR_FMT_MASK: instead of row_slot, 8 words per block whose bit i is set when row (first row + i) has entries in the
+//     block.  The sum of a row goes to rsw[q], q = its ordinal among the block's non-empty rows, which the row sums find
+//     from the ballots of the row ends and the epilogue from a prefix popcount of the mask.
+// Both change where bytes come from, not what is added: the products and every summation order are those of FMT 0.
+//
 // Summation order.  Inside a lane: strictly left to right.  A row that spans lanes is (carry from the earlier lanes) +
 // (this lane's left-to-right part).  Everything is a fixed function of the block cut, so results are bit-reproducible run
 // to run; they differ in the last bits from a sequential row sum (parity tests: 1e-12 relative, tests/test_gpu_parity.py).
@@ -43,6 +53,12 @@ __host__ __device__ constexpr int bicsr_min_ctas(int npre) { return npre > 1 ? 3
 
 __host__ __device__ constexpr int bicsr_slot(int q) { return (q % BICSR_CH) * 32 + q / BICSR_CH; }
 
+constexpr int BICSR_FMT_IDX3     = 1;        // three-byte block-local column indices (lo16 + hi8)
+constexpr int BICSR_FMT_MASK     = 2;        // non-empty-row mask instead of row_slot
+constexpr int BICSR_IDX3_MAX_WIDTH = 1 << 21;  // widest column block the three-byte indices can address
+constexpr unsigned BICSR_HI_PAD  = 0x40u;
+constexpr unsigned BICSR_HI_END  = 0x80u;
+
 struct bicsr_view_t {
   const int2* desc;                // n_blk block descriptors {first row, one past the last row}; long-row blocks: {row, row + 1}
   const unsigned short* row_slot;  // per row: slot (inside its block) of the row's last entry, BICSR_EMPTY for an empty row
@@ -52,22 +68,113 @@ struct bicsr_view_t {
   const int* off;                  // plain CSR of the same matrix: read by the long-row blocks only
   const int* cidx;
   const double* cval;
+  const unsigned short* lo16;      // BICSR_FMT_IDX3: n_std * 256 low halves of the local columns
+  const unsigned long long* hi8;   // BICSR_FMT_IDX3: n_std * 32 words of high bytes (one per lane)
+  const unsigned* mask;            // BICSR_FMT_MASK: n_std * 8 words
+  int col0;                        // BICSR_FMT_IDX3: first column of the column block
 };
 
+// Index words of one interleaved block, as the core keeps them between the load and the gathers.
+template <int FMT>
+struct bicsr_cols_t {
+  int c[BICSR_CH];  // FMT 0: stored index (bit 31: row end)
+};
+template <>
+struct bicsr_cols_t<BICSR_FMT_IDX3> {
+  uint4 lo;
+  unsigned long long hi;
+};
+template <>
+struct bicsr_cols_t<BICSR_FMT_IDX3 | BICSR_FMT_MASK> : bicsr_cols_t<BICSR_FMT_IDX3> {};
+template <>
+struct bicsr_cols_t<BICSR_FMT_MASK> : bicsr_cols_t<0> {};
+
+template <int FMT>
+__device__ __forceinline__ void bicsr_load_cols(const bicsr_view_t& A, int b, int lane, bicsr_cols_t<FMT>& w)
+{
+  if constexpr ((FMT & BICSR_FMT_IDX3) != 0) {
+    w.lo = __ldcs(reinterpret_cast<const uint4*>(A.lo16 + (size_t)b * BICSR_SLOTS) + lane);
+    w.hi = __ldcs(A.hi8 + (size_t)b * 32 + lane);
+  } else {
+#pragma unroll
+    for (int k = 0; k < BICSR_CH; ++k) w.c[k] = ld_stream(A.idx + (size_t)b * BICSR_SLOTS + k * 32 + lane);
+  }
+}
+// column of entry k, relative to the gather pointer (-1: unused slot)
+template <int FMT>
+__device__ __forceinline__ int bicsr_col(const bicsr_cols_t<FMT>& w, int k)
+{
+  if constexpr ((FMT & BICSR_FMT_IDX3) != 0) {
+    const unsigned lw = k < 2 ? w.lo.x : k < 4 ? w.lo.y : k < 6 ? w.lo.z : w.lo.w;
+    const unsigned hb = (unsigned)(w.hi >> (8 * k)) & 0xffu;
+    return (hb & BICSR_HI_PAD) ? -1 : (int)(((hb & 0x1fu) << 16) | ((lw >> (16 * (k & 1))) & 0xffffu));
+  } else {
+    const int col = w.c[k] & 0x7fffffff;
+    return col != BICSR_PAD ? col : -1;
+  }
+}
+// bit k: entry k closes a row
+template <int FMT>
+__device__ __forceinline__ unsigned bicsr_ends(const bicsr_cols_t<FMT>& w)
+{
+  unsigned ends = 0;
+#pragma unroll
+  for (int k = 0; k < BICSR_CH; ++k) {
+    if constexpr ((FMT & BICSR_FMT_IDX3) != 0) ends |= (unsigned)((w.hi >> (8 * k + 7)) & 1u) << k;
+    else ends |= (unsigned)(w.c[k] < 0) << k;
+  }
+  return ends;
+}
+template <int FMT>
+__device__ __forceinline__ const double* bicsr_gather_base(const bicsr_view_t& A, const double* x)
+{
+  if constexpr ((FMT & BICSR_FMT_IDX3) != 0) return x + A.col0;
+  else return x;
+}
+
+// Row epilogue lookup of BICSR_FMT_MASK: the block's mask word of row group q (mw: word `lane` of the block's mask in
+// lanes 0-7) gives this lane's row its ordinal among the non-empty rows; base counts the non-empty rows of groups < q.
+struct bicsr_mask_cursor_t {
+  unsigned mw;
+  int base;
+  // -1: this lane's row of group q is empty in the block
+  __device__ __forceinline__ int next(int q, int lane)
+  {
+    const unsigned m = __shfl_sync(0xffffffffu, mw, q);
+    const int ord    = ((m >> lane) & 1u) ? base + __popc(m & ((1u << lane) - 1u)) : -1;
+    base += __popc(m);
+    return ord;
+  }
+};
+
+// Row ends in the lanes before this one (BICSR_FMT_MASK): prefix popcount over the bits of the per-lane counts (<= 8: 4 ballots).
+__device__ __forceinline__ int bicsr_ends_before(unsigned ends, int lane)
+{
+  const unsigned cnt = __popc(ends), lt = (1u << lane) - 1u;
+  int before         = 0;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) before += __popc(__ballot_sync(0xffffffffu, (cnt >> j) & 1u) & lt) << j;
+  return before;
+}
+
 // Steps 3-4 of the core for one gathered vector: bit k of `ends` = entry k of this lane closes a row; the sum of every row
-// that ends in this lane's chunk goes to rsw[slot of its last entry].
+// that ends in this lane's chunk goes to rsw[slot of its last entry].  MASK (BICSR_FMT_MASK): to rsw[ordinal of the row
+// among the block's row ends] instead; before = bicsr_ends_before(ends, lane).
+template <bool MASK = false>
 __device__ __forceinline__ void bicsr_block_row_sums(const double (&a)[BICSR_CH], const double (&g)[BICSR_CH], unsigned ends,
-                                                     int lane, double* rsw)
+                                                     int lane, double* rsw, int before = 0)
 {
   constexpr unsigned FULL = 0xffffffffu;
   // chunk sums, left to right, branch-free; the FIRST row end of the chunk still lacks what earlier lanes hold of that row
   double s = 0.0, head = 0.0;
   const int kf = ends ? __ffs(ends) - 1 : -1;
+  int ord      = before;  // MASK: ordinal of the next row end
 #pragma unroll
   for (int k = 0; k < BICSR_CH; ++k) {
     s = __dadd_rn(s, __dmul_rn(a[k], g[k]));  // product, then sum: no FMA contraction (the CPU oracle has none either)
     const bool e = (ends >> k) & 1u;
-    if (e && k != kf) rsw[k * 32 + lane] = s;
+    if (e && k != kf) rsw[MASK ? ord : k * 32 + lane] = s;
+    if constexpr (MASK) ord += e;
     head = (k == kf) ? s : head;
     s    = e ? 0.0 : s;
   }
@@ -83,7 +190,7 @@ __device__ __forceinline__ void bicsr_block_row_sums(const double (&a)[BICSR_CH]
     if (lane == 0) carry = 0.0;
     pending &= pending << 1;
   }
-  if (kf >= 0) rsw[kf * 32 + lane] = carry + head;
+  if (kf >= 0) rsw[MASK ? before : kf * 32 + lane] = carry + head;
 }
 
 // Walks this warp's blocks.
@@ -95,7 +202,8 @@ __device__ __forceinline__ void bicsr_block_row_sums(const double (&a)[BICSR_CH]
 // blocked product (pdlp_kernels.cuh).
 // NPRE: row groups (of 32 rows) per block whose payload is fetched ahead of the gathers: 1, or 2 for matrices with short
 // rows, whose blocks hold ~64 rows (the column blocks of a gather-blocked matrix: 4 entries per row at configs[3]).
-template <typename P, bool INIT = false, int NPRE = 1, typename PreOp, typename RowOp>
+// FMT: storage form of the interleaved blocks (BICSR_FMT_* bits, 0 = plain).
+template <typename P, bool INIT = false, int NPRE = 1, int FMT = 0, typename PreOp, typename RowOp>
 __device__ __forceinline__ void spmv_bicsr_rows(const bicsr_view_t& A,
                                                 const double* __restrict__ x,
                                                 double* rsw,
@@ -103,25 +211,25 @@ __device__ __forceinline__ void spmv_bicsr_rows(const bicsr_view_t& A,
                                                 RowOp& row_op,
                                                 unsigned long long gather_policy)
 {
+  constexpr bool MASK     = (FMT & BICSR_FMT_MASK) != 0;
   const int lane          = threadIdx.x & 31;
   const int gwarp         = blockIdx.x * BICSR_WARPS + (threadIdx.x >> 5);
   const int nwarps        = gridDim.x * BICSR_WARPS;
-  int c[BICSR_CH];
-  if (gwarp < A.n_std) {
-#pragma unroll
-    for (int k = 0; k < BICSR_CH; ++k) c[k] = ld_stream(A.idx + (size_t)gwarp * BICSR_SLOTS + k * 32 + lane);
-  }
+  const double* xg        = bicsr_gather_base<FMT>(A, x);
+  bicsr_cols_t<FMT> c;
+  if (gwarp < A.n_std) bicsr_load_cols<FMT>(A, gwarp, lane, c);
   for (int b = gwarp; b < A.n_std; b += nwarps) {
     const int2 d  = __ldg(A.desc + b);
     const int r0 = d.x, r1 = d.y;
     P pl[NPRE];
     unsigned short slot[NPRE];
+    bicsr_mask_cursor_t mc{0u, 0};
 #pragma unroll
     for (int q = 0; q < NPRE; ++q) {
       slot[q] = BICSR_EMPTY;
       if (r0 + lane + 32 * q < r1) {
-        pl[q]   = pre_op(r0 + lane + 32 * q);
-        slot[q] = __ldg(A.row_slot + r0 + lane + 32 * q);
+        pl[q] = pre_op(r0 + lane + 32 * q);
+        if constexpr (!MASK) slot[q] = __ldg(A.row_slot + r0 + lane + 32 * q);
       }
     }
     const size_t base = (size_t)b * BICSR_SLOTS + lane;
@@ -130,32 +238,38 @@ __device__ __forceinline__ void spmv_bicsr_rows(const bicsr_view_t& A,
     for (int k = 0; k < BICSR_CH; ++k) a[k] = ld_stream(A.val + base + k * 32);
 #pragma unroll
     for (int k = 0; k < BICSR_CH; ++k) {
-      const int col = c[k] & 0x7fffffff;
-      g[k]          = col != BICSR_PAD ? ld_l2(x + col, gather_policy) : 0.0;
+      const int col = bicsr_col<FMT>(c, k);
+      g[k]          = col >= 0 ? ld_l2(xg + col, gather_policy) : 0.0;
     }
-    unsigned ends = 0;
-#pragma unroll
-    for (int k = 0; k < BICSR_CH; ++k) ends |= (unsigned)(c[k] < 0) << k;
-    if (b + nwarps < A.n_std) {
-#pragma unroll
-      for (int k = 0; k < BICSR_CH; ++k) c[k] = ld_stream(A.idx + (size_t)(b + nwarps) * BICSR_SLOTS + k * 32 + lane);
-    }
-    bicsr_block_row_sums(a, g, ends, lane, rsw);
+    if constexpr (MASK) mc.mw = lane < 8 ? __ldg(A.mask + (size_t)b * 8 + lane) : 0u;  // after the gathers: fewer live registers
+    const unsigned ends = bicsr_ends<FMT>(c);
+    if (b + nwarps < A.n_std) bicsr_load_cols<FMT>(A, b + nwarps, lane, c);
+    bicsr_block_row_sums<MASK>(a, g, ends, lane, rsw, MASK ? bicsr_ends_before(ends, lane) : 0);
     __syncwarp();
 #pragma unroll
     for (int q = 0; q < NPRE; ++q) {
+      int src = slot[q] != BICSR_EMPTY ? (int)slot[q] : -1;
+      if constexpr (MASK) src = mc.next(q, lane);
       if (r0 + lane + 32 * q < r1) {
-        double sum = slot[q] != BICSR_EMPTY ? rsw[slot[q]] : 0.0;
+        double sum = src >= 0 ? rsw[src] : 0.0;
         if constexpr (INIT) sum = pl[q].init + sum;
         row_op(r0 + lane + 32 * q, sum, pl[q]);
       }
     }
-    for (int r = r0 + 32 * NPRE + lane; r < r1; r += 32) {  // blocks of very short rows hold more rows still
-      const P p2              = pre_op(r);
-      const unsigned short s2 = __ldg(A.row_slot + r);
-      double sum              = s2 != BICSR_EMPTY ? rsw[s2] : 0.0;
-      if constexpr (INIT) sum = p2.init + sum;
-      row_op(r, sum, p2);
+    for (int q = NPRE; 32 * q < r1 - r0; ++q) {  // blocks of very short rows hold more rows still
+      const int r = r0 + 32 * q + lane;
+      int src     = -1;
+      if constexpr (MASK) src = mc.next(q, lane);
+      if (r < r1) {
+        const P p2 = pre_op(r);
+        if constexpr (!MASK) {
+          const unsigned short s2 = __ldg(A.row_slot + r);
+          src                     = s2 != BICSR_EMPTY ? (int)s2 : -1;
+        }
+        double sum = src >= 0 ? rsw[src] : 0.0;
+        if constexpr (INIT) sum = p2.init + sum;
+        row_op(r, sum, p2);
+      }
     }
     __syncwarp();
   }
@@ -179,7 +293,7 @@ __device__ __forceinline__ void spmv_bicsr_rows(const bicsr_view_t& A,
 // in spmv_bicsr_rows.  Each sum is formed exactly as spmv_bicsr_rows forms it.  rsw_u / rsw_v: BICSR_SLOTS doubles each.
 // No payload is fetched ahead and the next block's indices are not prefetched: the 16 gathers of a block already keep the
 // warp's loads in flight, and the registers go to the second set of gathered values.
-template <typename RowOp>
+template <int FMT = 0, typename RowOp>
 __device__ __forceinline__ void spmv_bicsr_rows_pair(const bicsr_view_t& A,
                                                      const double* __restrict__ u,
                                                      const double* __restrict__ v,
@@ -188,33 +302,44 @@ __device__ __forceinline__ void spmv_bicsr_rows_pair(const bicsr_view_t& A,
                                                      RowOp& row_op,
                                                      unsigned long long gather_policy)
 {
+  constexpr bool MASK = (FMT & BICSR_FMT_MASK) != 0;
   const int lane   = threadIdx.x & 31;
   const int gwarp  = blockIdx.x * BICSR_WARPS + (threadIdx.x >> 5);
   const int nwarps = gridDim.x * BICSR_WARPS;
+  const double* ug = bicsr_gather_base<FMT>(A, u);
+  const double* vg = bicsr_gather_base<FMT>(A, v);
   for (int b = gwarp; b < A.n_std; b += nwarps) {
     const int2 d      = __ldg(A.desc + b);
     const size_t base = (size_t)b * BICSR_SLOTS + lane;
-    int c[BICSR_CH];
+    bicsr_cols_t<FMT> c;
     double a[BICSR_CH], gu[BICSR_CH], gv[BICSR_CH];
-#pragma unroll
-    for (int k = 0; k < BICSR_CH; ++k) c[k] = ld_stream(A.idx + base + k * 32);
+    bicsr_load_cols<FMT>(A, b, lane, c);
+    bicsr_mask_cursor_t mc{0u, 0};
 #pragma unroll
     for (int k = 0; k < BICSR_CH; ++k) a[k] = ld_stream(A.val + base + k * 32);
 #pragma unroll
     for (int k = 0; k < BICSR_CH; ++k) {
-      const int col = c[k] & 0x7fffffff;
-      gu[k]         = col != BICSR_PAD ? ld_l2(u + col, gather_policy) : 0.0;
-      gv[k]         = col != BICSR_PAD ? ld_l2(v + col, gather_policy) : 0.0;
+      const int col = bicsr_col<FMT>(c, k);
+      gu[k]         = col >= 0 ? ld_l2(ug + col, gather_policy) : 0.0;
+      gv[k]         = col >= 0 ? ld_l2(vg + col, gather_policy) : 0.0;
     }
-    unsigned ends = 0;
-#pragma unroll
-    for (int k = 0; k < BICSR_CH; ++k) ends |= (unsigned)(c[k] < 0) << k;
-    bicsr_block_row_sums(a, gu, ends, lane, rsw_u);
-    bicsr_block_row_sums(a, gv, ends, lane, rsw_v);
+    const unsigned ends = bicsr_ends<FMT>(c);
+    const int before    = MASK ? bicsr_ends_before(ends, lane) : 0;
+    bicsr_block_row_sums<MASK>(a, gu, ends, lane, rsw_u, before);
+    bicsr_block_row_sums<MASK>(a, gv, ends, lane, rsw_v, before);
+    if constexpr (MASK) mc.mw = lane < 8 ? __ldg(A.mask + (size_t)b * 8 + lane) : 0u;  // two sets of gathers hold the registers
     __syncwarp();
-    for (int r = d.x + lane; r < d.y; r += 32) {
-      const unsigned short s = __ldg(A.row_slot + r);
-      row_op(r, s != BICSR_EMPTY ? rsw_u[s] : 0.0, s != BICSR_EMPTY ? rsw_v[s] : 0.0);
+    for (int q = 0; 32 * q < d.y - d.x; ++q) {
+      const int r = d.x + 32 * q + lane;
+      int s       = -1;
+      if constexpr (MASK) s = mc.next(q, lane);
+      if (r < d.y) {
+        if constexpr (!MASK) {
+          const unsigned short s2 = __ldg(A.row_slot + r);
+          s                       = s2 != BICSR_EMPTY ? (int)s2 : -1;
+        }
+        row_op(r, s >= 0 ? rsw_u[s] : 0.0, s >= 0 ? rsw_v[s] : 0.0);
+      }
     }
     __syncwarp();
   }
@@ -290,6 +415,58 @@ __global__ void __launch_bounds__(256) k_bicsr_fill_values(int n_std,
       const int q                = BICSR_CH * lane + k;
       bval[base + k * 32 + lane] = q < cnt ? val[lo + q] : 0.0;
     }
+  }
+}
+
+// Structure of a column block in a compact form, from its plain CSR (values: k_bicsr_fill; the plain idx / row_slot arrays
+// stay for the parts of the form that are not compact).  Null outputs are not written: lo16 / hi8 (BICSR_FMT_IDX3, columns
+// relative to col0), mask (BICSR_FMT_MASK).
+__global__ void __launch_bounds__(BICSR_THREADS) k_bicsr_fill_structure(int n_std,
+                                                                      const int2* __restrict__ desc,
+                                                                      const int* __restrict__ off,
+                                                                      const int* __restrict__ idx,
+                                                                      int col0,
+                                                                      unsigned short* __restrict__ lo16,
+                                                                      unsigned long long* __restrict__ hi8,
+                                                                      unsigned* __restrict__ mask)
+{
+  __shared__ unsigned char is_end[BICSR_WARPS][BICSR_SLOTS];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  unsigned char* e = is_end[w];
+  for (int b = blockIdx.x * BICSR_WARPS + w; b < n_std; b += gridDim.x * BICSR_WARPS) {
+    const int2 d      = desc[b];
+    const int lo      = off[d.x];
+    const int cnt     = off[d.y] - lo;
+    const size_t base = (size_t)b * BICSR_SLOTS;
+#pragma unroll
+    for (int k = 0; k < BICSR_CH; ++k) e[BICSR_CH * lane + k] = 0;
+    __syncwarp();
+    for (int q = 0; q < BICSR_MAX_ROWS / 32; ++q) {  // warp-uniform: the ballot needs every lane
+      const int r  = d.x + 32 * q + lane;
+      const int p0 = r < d.y ? off[r] : 0, p1 = r < d.y ? off[r + 1] : 0;
+      if (p1 > p0) e[p1 - 1 - lo] = 1;
+      const unsigned word = __ballot_sync(0xffffffffu, p1 > p0);
+      if (mask && lane == 0) mask[(size_t)b * 8 + q] = word;
+    }
+    __syncwarp();
+    if (lo16) {
+      unsigned lw[4] = {0u, 0u, 0u, 0u};
+      unsigned long long hw = 0ull;
+#pragma unroll
+      for (int k = 0; k < BICSR_CH; ++k) {
+        const int q = BICSR_CH * lane + k;
+        unsigned hb = BICSR_HI_PAD;
+        if (q < cnt) {
+          const unsigned c = (unsigned)(idx[lo + q] - col0);
+          lw[k / 2] |= (c & 0xffffu) << (16 * (k & 1));
+          hb = (c >> 16) | (e[q] ? BICSR_HI_END : 0u);
+        }
+        hw |= (unsigned long long)hb << (8 * k);
+      }
+      reinterpret_cast<uint4*>(lo16 + base)[lane] = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+      hi8[(size_t)b * 32 + lane]                  = hw;
+    }
+    __syncwarp();
   }
 }
 
