@@ -75,7 +75,7 @@ REFERENCE_SYMBOLS = [
 EXTENSION_SYMBOLS = [
     "cuOptB200GetLPStats", "cuOptB200SolverCreate", "cuOptB200SolverDestroy", "cuOptB200SolverInitialise",
     "cuOptB200SolverAdvance", "cuOptB200SolverGetScalar", "cuOptB200SolverGetVector", "cuOptB200SolverGetSolution",
-    "cuOptB200SolverTrustRegionBounds",
+    "cuOptB200SolverTrustRegionBounds", "cuOptB200SolverInfeasibilityStats",
     "cuOptB200SolverProfileKernels", "cuOptB200ReadProblem", "cuOptB200Version", "cuOptB200DistGetUniqueId",
     "cuOptB200DistInit", "cuOptB200DistDestroy", "cuOptB200SolveDistributed",
     "cuOptB200SetWarmStartCapture", "cuOptB200GetWarmStart", "cuOptB200SetWarmStart", "cuOptB200CreateWarmStart",
@@ -161,6 +161,7 @@ def lib():
         L.cuOptB200SolverGetVector.argtypes = [vp, C.c_char_p, c_dbl_p, C.c_int32, c_int_p]
         L.cuOptB200SolverGetSolution.argtypes = [vp, C.POINTER(vp)]
         L.cuOptB200SolverTrustRegionBounds.argtypes = [vp, c_dbl_p, c_dbl_p, C.c_double, c_dbl_p, c_dbl_p]
+        L.cuOptB200SolverInfeasibilityStats.argtypes = [vp, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_dbl_p, c_int_p]
         L.cuOptB200SolverProfileKernels.argtypes = [vp, C.c_int32, C.c_int32, C.POINTER(KernelProfile)]
         L.cuOptB200ReadProblem.argtypes = [C.c_char_p, C.c_int32, C.POINTER(vp)]
         L.cuOptB200Version.restype = C.c_char_p
@@ -514,6 +515,21 @@ class Solver:
         _check(lib().cuOptB200SolverTrustRegionBounds(self.h, _dp(px), _dp(py), float(radius), C.byref(lo), C.byref(up)),
                "trust_region_bounds")
         return lo.value, up.value
+
+    INFEASIBILITY_STATS = ("xinf", "max_viol", "hres", "cx", "yinf", "rcinf", "hdres_raw", "dobj_raw", "pobj",
+                           "max_primal", "hdres", "dobj")
+
+    def infeasibility_stats(self, x_cur, y_cur, x_avg, y_avg):
+        """(stats, status): the 12 detection statistics of the current and the average point (a 2 x 12 array in the order
+        of INFEASIBILITY_STATS) and the verdict each would draw (2, 3 or 6), at points of the unscaled minimisation form
+        of the original problem; changes no state."""
+        pts = [np.ascontiguousarray(v, np.float64) for v in (x_cur, y_cur, x_avg, y_avg)]
+        if any(len(v) != (self.n if k % 2 == 0 else self.m) for k, v in enumerate(pts)):
+            raise ValueError(f"expected {self.n} primal and {self.m} dual values per point")
+        stats, status = np.zeros((2, 12)), (C.c_int32 * 2)()
+        _check(lib().cuOptB200SolverInfeasibilityStats(self.h, *(_dp(v) for v in pts), _dp(stats), status),
+               "infeasibility_stats")
+        return stats, [status[0], status[1]]
 
     def solution(self) -> Solution:
         h = C.c_void_p()

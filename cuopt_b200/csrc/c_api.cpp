@@ -817,6 +817,25 @@ cuopt_int_t cuOptB200SolverTrustRegionBounds(cuOptB200Solver solver,
   SOLVER_GUARD(static_cast<solver_handle_t*>(solver)->solver->trust_region_bounds(px, py, radius, *lower_ptr, *upper_ptr));
   return CUOPT_SUCCESS;
 }
+cuopt_int_t cuOptB200SolverInfeasibilityStats(cuOptB200Solver solver,
+                                              const cuopt_float_t* x_cur,
+                                              const cuopt_float_t* y_cur,
+                                              const cuopt_float_t* x_avg,
+                                              const cuopt_float_t* y_avg,
+                                              cuopt_float_t* stats,
+                                              cuopt_int_t* status)
+{
+  if (solver == nullptr || x_cur == nullptr || y_cur == nullptr || x_avg == nullptr || y_avg == nullptr ||
+      stats == nullptr || status == nullptr)
+    return CUOPT_INVALID_ARGUMENT;
+  SOLVER_GUARD({
+    int st[2];
+    static_cast<solver_handle_t*>(solver)->solver->infeasibility_stats(x_cur, y_cur, x_avg, y_avg, stats, st);
+    status[0] = st[0];
+    status[1] = st[1];
+  });
+  return CUOPT_SUCCESS;
+}
 cuopt_int_t cuOptB200SolverGetSolution(cuOptB200Solver solver, cuOptSolution* solution_ptr)
 {
   if (solver == nullptr || solution_ptr == nullptr) return CUOPT_INVALID_ARGUMENT;

@@ -1139,7 +1139,10 @@ __global__ void __launch_bounds__(EW_THREADS) k_infeasibility_rows(int m,
 }
 // columns -> parts (12 x gridDim.x): max |x|, max bound violation of the ray, max |g - rc|, max |rc| (max), c.x,
 // sum bound_value_product(rc) (sum), each x {cur, avg}; g = -A^T y.  Last CTA: compute_remaining_stats_kernel
-// (:118-181) + the two tests.
+// (:118-181) + the two tests.  stats_out (nullable; null in the solve) receives INFEAS_STATS doubles per iterate:
+// xinf, max_viol, hres, c.x, yinf, rcinf, hdres, dobj, pobj, max_primal, hdres / scaling, dobj / scaling, and the status
+// the tests give (2, 3 or 6), for cuOptB200SolverInfeasibilityStats.
+constexpr int INFEAS_STATS = 13;
 __global__ void __launch_bounds__(EW_THREADS) k_infeasibility_cols(pdhg_ctl_t* __restrict__ ctl,
                                                                    int n,
                                                                    const double* __restrict__ aty_cur,
@@ -1153,7 +1156,8 @@ __global__ void __launch_bounds__(EW_THREADS) k_infeasibility_cols(pdhg_ctl_t* _
                                                                    const double* __restrict__ parts_rows,
                                                                    int n_parts_rows,
                                                                    eval_consts_t k,
-                                                                   eval_t* __restrict__ out)
+                                                                   eval_t* __restrict__ out,
+                                                                   double* __restrict__ stats_out)
 {
   __shared__ double red[32];
   __shared__ bool is_last;
@@ -1228,8 +1232,15 @@ __global__ void __launch_bounds__(EW_THREADS) k_infeasibility_cols(pdhg_ctl_t* _
       max_primal = 0.0;
       pobj       = 0.0;
     }
-    if (dobj > 0.0 && hdres / dobj <= k.primal_infeasible_tol) out[v].status = 2;
-    else if (pobj < 0.0 && max_primal / -pobj <= k.dual_infeasible_tol) out[v].status = 3;
+    int status = 6;
+    if (dobj > 0.0 && hdres / dobj <= k.primal_infeasible_tol) status = 2;
+    else if (pobj < 0.0 && max_primal / -pobj <= k.dual_infeasible_tol) status = 3;
+    if (status != 6) out[v].status = status;
+    if (stats_out != nullptr) {
+      const double s[INFEAS_STATS] = {xinf, max_viol, hres, csum[0 + v], yinf, rcinf, cmax[4 + v], rsum[v] + csum[2 + v],
+                                      pobj, max_primal, hdres, dobj, (double)status};
+      for (int q = 0; q < INFEAS_STATS; ++q) stats_out[v * INFEAS_STATS + q] = s[q];
+    }
   }
 }
 

@@ -1684,7 +1684,7 @@ struct pdlp_solver_t::impl_t {
                                                                 y_avg.data(), lc.data(), uc.data(), rows_parts);
         k_infeasibility_cols<<<grid_n, EW_THREADS, 0, stream>>>(d_ctl.data(), n, aty2, aty2 + n, xbuf[cur].data(),
                                                                 x_avg.data(), c.data(), l.data(), u.data(), cols_parts,
-                                                                rows_parts, grid_m, eval_consts(), d_eval.data());
+                                                                rows_parts, grid_m, eval_consts(), d_eval.data(), nullptr);
         launches += 2;
       }
     }
@@ -1704,7 +1704,7 @@ struct pdlp_solver_t::impl_t {
     sol.stats.solved_by_pdlp = 0;
     if (ps.verdict == termination_status_t::Optimal) {
       const double t0 = now_seconds();
-      postsolve_device(ps, {}, {}, {}, false, sol.primal, sol.dual, sol.reduced_cost, stream);
+      postsolve_device(ps, {}, {}, {}, false, false, sol.primal, sol.dual, sol.reduced_cost, stream);
       ps.stats.postsolve_seconds = now_seconds() - t0;
       const double obj           = obj_scale * ps.offset + obj_offset;
       sol.stats.primal_objective = obj;
@@ -1718,7 +1718,8 @@ struct pdlp_solver_t::impl_t {
     initialised = finished = postsolved = true;
   }
   // Every ending of a presolved solve: the reduced-space vectors fill_solution / fill_best_solution left in sol go back to
-  // the original sizes.  Infeasibility verdicts carry certificates: scattered, zeros elsewhere.  When presolve removed nothing
+  // the original sizes.  Infeasibility verdicts carry certificates: scattered, zeros elsewhere, except that a dual ray gives
+  // the singleton rows the duals of the bounds they supplied.  When presolve removed nothing
   // the vectors are already those of the original problem.  An ending without vectors (NumericalError) keeps none.
   void postsolve_solution()
   {
@@ -1730,7 +1731,8 @@ struct pdlp_solver_t::impl_t {
     if (!ps.removed_nothing() && !(sol.primal.empty() && sol.dual.empty())) {
       CUOPT_CUDA_TRY(cudaEventRecord(ev_a, stream));
       std::vector<double> x, y, r;
-      postsolve_device(ps, sol.primal, sol.dual, sol.reduced_cost, certificate, x, y, r, stream);
+      postsolve_device(ps, sol.primal, sol.dual, sol.reduced_cost, certificate,
+                       sol.termination_status == termination_status_t::PrimalInfeasible, x, y, r, stream);
       CUOPT_CUDA_TRY(cudaEventRecord(ev_b, stream));
       CUOPT_CUDA_TRY(cudaEventSynchronize(ev_b));
       float ms = 0.f;
@@ -1982,6 +1984,39 @@ struct pdlp_solver_t::impl_t {
     launches = count;
     lower    = g.lower;
     upper    = g.upper;
+  }
+  // The detection statistics of evaluate_iterates at caller-given current / average points (unscaled; reduced problem when
+  // presolved), through the evaluation's own products and kernels (cuOptB200SolverInfeasibilityStats).  Every buffer
+  // written is local; the column pass takes ticket[3] of d_ctl, which its last CTA returns to 0.
+  void infeasibility_stats_at(const double* hx_cur, const double* hy_cur, const double* hx_avg, const double* hy_avg,
+                              double* stats, int* status)
+  {
+    dvec<double> px(2 * (size_t)n), py(2 * (size_t)m), ax(2 * (size_t)m), aty(2 * (size_t)n), out(2 * INFEAS_STATS);
+    dvec<double> parts(6 * (size_t)grid_m + 12 * (size_t)grid_n);
+    CUOPT_CUDA_TRY(cudaMemcpyAsync(px.data(), hx_cur, n * sizeof(double), cudaMemcpyHostToDevice, stream));
+    CUOPT_CUDA_TRY(cudaMemcpyAsync(px.data() + n, hx_avg, n * sizeof(double), cudaMemcpyHostToDevice, stream));
+    CUOPT_CUDA_TRY(cudaMemcpyAsync(py.data(), hy_cur, m * sizeof(double), cudaMemcpyHostToDevice, stream));
+    CUOPT_CUDA_TRY(cudaMemcpyAsync(py.data() + m, hy_avg, m * sizeof(double), cudaMemcpyHostToDevice, stream));
+    eval_t h_keep[2] = {};
+    h_keep[0].status = h_keep[1].status = 6;
+    dvec<eval_t> keep(2);
+    CUOPT_CUDA_TRY(cudaMemcpyAsync(keep.data(), h_keep, sizeof(h_keep), cudaMemcpyHostToDevice, stream));
+    launch_spmv_pair(A, blkA, px.data(), px.data() + n, ax.data(), ax.data() + m);
+    launch_spmv_pair(AT, blkAT, py.data(), py.data() + m, aty.data(), aty.data() + n);
+    k_infeasibility_rows<<<grid_m, EW_THREADS, 0, stream>>>(m, ax.data(), ax.data() + m, py.data(), py.data() + m,
+                                                            lc.data(), uc.data(), parts.data());
+    k_infeasibility_cols<<<grid_n, EW_THREADS, 0, stream>>>(d_ctl.data(), n, aty.data(), aty.data() + n, px.data(),
+                                                            px.data() + n, c.data(), l.data(), u.data(),
+                                                            parts.data() + 6 * (size_t)grid_m, parts.data(), grid_m,
+                                                            eval_consts(), keep.data(), out.data());
+    check_launch();
+    double h[2 * INFEAS_STATS];
+    out.download(h, stream);
+    sync();
+    for (int v = 0; v < 2; ++v) {
+      for (int q = 0; q < INFEAS_STATS - 1; ++q) stats[v * (INFEAS_STATS - 1) + q] = h[v * INFEAS_STATS + q];
+      status[v] = (int)h[v * INFEAS_STATS + INFEAS_STATS - 1];
+    }
   }
   void trust_region_restart()  // pdlp_restart_strategy.cu:278-364
   {
@@ -2293,6 +2328,16 @@ void pdlp_solver_t::trust_region_bounds(const double* px, const double* py, doub
   if (!(radius >= 0.0)) throw lp_error(error_type_t::InvalidArgument, "trust-region radius must be >= 0");
   s.fetch_ctl();
   s.trust_region_bounds_at(px, py, radius, lower, upper);
+}
+
+void pdlp_solver_t::infeasibility_stats(const double* x_cur, const double* y_cur, const double* x_avg,
+                                        const double* y_avg, double* stats, int* status)
+{
+  impl_t& s = *impl_;
+  if (s.sharded()) throw lp_error(error_type_t::InvalidArgument, "infeasibility statistics are not available in multi-GPU sessions");
+  if (!s.initialised || s.d_ctl.size() == 0)
+    throw lp_error(error_type_t::InvalidArgument, "infeasibility statistics need an initialised session");
+  s.infeasibility_stats_at(x_cur, y_cur, x_avg, y_avg, stats, status);
 }
 
 kernel_profile_t pdlp_solver_t::profile_kernels(int warmup_steps, int reps)

@@ -44,6 +44,10 @@ class pdlp_solver_t {
   // Lower / upper bound of the trust-region restart (Methodical1) at a point (px: n, py: m values) of the scaled space,
   // radius >= 0; reads the solver state, changes none of it.
   void trust_region_bounds(const double* px, const double* py, double radius, double& lower, double& upper);
+  // Infeasibility-detection statistics (12 per iterate) and the status the tests give, at current / average points of the
+  // unscaled minimisation form (x: n, y: m values); reads the solver state, changes none of it.
+  void infeasibility_stats(const double* x_cur, const double* y_cur, const double* x_avg, const double* y_avg,
+                           double* stats, int* status);
   const lp_solution_t& solution() const;
 
   struct impl_t;

@@ -453,8 +453,8 @@ void presolve_device(int& m, int& n, dvec<int>& off, dvec<int>& idx, dvec<double
 }
 
 void postsolve_device(const presolve_state_t& ps, const std::vector<double>& x_red, const std::vector<double>& y_red,
-                      const std::vector<double>& rc_red, bool certificate, std::vector<double>& x, std::vector<double>& y,
-                      std::vector<double>& rc, cudaStream_t s)
+                      const std::vector<double>& rc_red, bool certificate, bool dual_ray, std::vector<double>& x,
+                      std::vector<double>& y, std::vector<double>& rc, cudaStream_t s)
 {
   const int sms = device_sms();
   const int m = ps.m0, n = ps.n0;
@@ -474,6 +474,19 @@ void postsolve_device(const presolve_state_t& ps, const std::vector<double>& x_r
     if (!rc_red.empty())
       CUOPT_CUDA_TRY(cudaMemcpyAsync(rr.data(), rc_red.data(), rc_red.size() * sizeof(double), cudaMemcpyHostToDevice, s));
     k_pst_scatter<<<gn, PS_THREADS, 0, s>>>(n, ps.col_alive.data(), ps.col_new.data(), rr.data(), nullptr, r.data());
+    dvec<double> zero, r0;
+    if (dual_ray) {
+      // A bound a singleton row supplied is part of the reduced problem's ray objective; the row's dual carries it back
+      // to the original problem (the optimal ending's rule, with the gradient r0 = -A^T y of the ray: zero cost)
+      const int wn = grid_warps(n, sms);
+      zero.resize(n);
+      r0.resize(n);
+      zero.zero(s);
+      k_pst_reduced_cost<<<wn, PS_THREADS, 0, s>>>(n, ps.toff.data(), ps.tidx.data(), ps.tval.data(), zero.data(),
+                                                   yf.data(), r0.data());
+      k_pst_singleton_duals<<<gn, PS_THREADS, 0, s>>>(n, r0.data(), ps.src_lo.data(), ps.src_hi.data(), ps.a_lo.data(),
+                                                      ps.a_hi.data(), yf.data());
+    }
     CUOPT_CUDA_TRY(cudaStreamSynchronize(s));
   } else {
     const int wn = grid_warps(n, sms);

@@ -37,11 +37,13 @@ void presolve_device(int& m, int& n, dvec<int>& off, dvec<int>& idx, dvec<double
                      cudaStream_t stream, bool trace);
 
 // Postsolve of a reduced-space solution (host vectors of the reduced sizes, empty when there is none) into original-size
-// host vectors.  certificate: the vectors are an infeasibility certificate — scattered, zeros on the removed entries, no dual
-// recovery.  Otherwise removed columns take their fixed value, removed rows dual 0, the singleton rows that supply an active
-// bound get the dual that zeroes the column's reduced cost, and r = c - A^T y with the original A^T.
+// host vectors.  certificate: the vectors are an infeasibility certificate — scattered, zeros on the removed entries; with
+// dual_ray (a PrimalInfeasible ending) the singleton rows then get the duals that carry the bounds they supplied into the
+// ray's objective on the original problem (r0 = -A^T y in the rule below).  Otherwise removed columns take their fixed
+// value, removed rows dual 0, the singleton rows that supply an active bound get the dual that zeroes the column's reduced
+// cost, and r = c - A^T y with the original A^T.
 void postsolve_device(const presolve_state_t& ps, const std::vector<double>& x_red, const std::vector<double>& y_red,
-                      const std::vector<double>& rc_red, bool certificate, std::vector<double>& x, std::vector<double>& y,
-                      std::vector<double>& rc, cudaStream_t stream);
+                      const std::vector<double>& rc_red, bool certificate, bool dual_ray, std::vector<double>& x,
+                      std::vector<double>& y, std::vector<double>& rc, cudaStream_t stream);
 
 }  // namespace cuopt_b200

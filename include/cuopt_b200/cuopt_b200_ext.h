@@ -130,6 +130,24 @@ cuopt_int_t cuOptB200SolverTrustRegionBounds(cuOptB200Solver solver,
                                              cuopt_float_t radius,
                                              cuopt_float_t* lower_ptr,
                                              cuopt_float_t* upper_ptr);
+/* Read-only: the infeasibility-detection statistics of the termination check at a caller-given current point (x_cur,
+ * y_cur) and average point (x_avg, y_avg), from the products and kernels the evaluation runs.  The points are in the space
+ * the evaluation works in: unscaled, minimisation form (c negated when maximising), and of the reduced problem in a
+ * presolved session (x: num_variables values, y: num_constraints values).  stats receives 12 values per iterate, current
+ * first: max |x|, max bound violation of the ray, max homogeneous row violation, c.x, max |y|, max |reduced cost|, dual
+ * residual and dual-ray objective as summed, primal-ray objective c.x / max |x|, max primal residual / max |x|, and the
+ * dual residual and dual-ray objective divided by max(max |y|, max |reduced cost|); status receives the verdict of each
+ * iterate as the solve would draw it (2 PrimalInfeasible, 3 DualInfeasible, 6 none) under the session's
+ * primal_infeasible_tolerance, dual_infeasible_tolerance and reduced-cost rule.  Works whether or not
+ * infeasibility_detection is set; refused with CUOPT_INVALID_ARGUMENT before cuOptB200SolverInitialise and in multi-GPU
+ * sessions.  The iterates, the statistics and the launch count of the session are not changed. */
+cuopt_int_t cuOptB200SolverInfeasibilityStats(cuOptB200Solver solver,
+                                              const cuopt_float_t* x_cur,
+                                              const cuopt_float_t* y_cur,
+                                              const cuopt_float_t* x_avg,
+                                              const cuopt_float_t* y_avg,
+                                              cuopt_float_t* stats,
+                                              cuopt_int_t* status);
 /* Solution object (same type cuOptSolve returns) of a finished session. */
 cuopt_int_t cuOptB200SolverGetSolution(cuOptB200Solver solver, cuOptSolution* solution_ptr);
 /* Time the three PDHG kernels in situ (CUDA events on the solver's stream) after `warmup_steps`. */

@@ -796,19 +796,34 @@ def test_full_solve_reaches_planted_optimum(name, mode):
     assert np.all(np.abs(x[fixed] - lp.var_lb[fixed]) <= slack(lp.var_lb)[fixed])
 
 
+# Every preset under the strict rule; Stable2 under the non-strict rule too (Fast1's current and average iterates do not
+# cross the threshold at the same major iteration on the unbounded cases within CERT_CAP, measured on an H100).
+# Stable1 runs good-mps-free-var and good-mps-lower-bound-inf-var to the iteration limit (its iterate neither overflows
+# nor passes the ray test within CERT_CAP, as the oracle shows), so those two are left out under Stable1.
+VERDICT_CASES = [(n, m, strict) for n in CERTIFICATES for m in MODES for strict in (False, True)
+                 if (strict or m == po.STABLE2)
+                 and not (m == po.STABLE1 and n in ("good-mps-free-var", "good-mps-lower-bound-inf-var"))]
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("strict", [False, True])
-@pytest.mark.parametrize("name", CERTIFICATES)
-def test_certificate_verdict(name, strict):
+@pytest.mark.parametrize("name,mode,strict", VERDICT_CASES)
+def test_certificate_verdict(name, mode, strict):
+    """The verdict under every preset, and the returned vectors re-evaluated on the LP by the exact restatement of
+    test_infeasibility_detection with the preset's reduced-cost rule: they meet the criterion the solver reported."""
     from test_infeasibility import close_counts
+    from test_infeasibility_detection import LP, certifies
     off, idx, val, c, l, u, lc, uc = certificate_args(name)
     p = capi.Problem.create_ranged(off, idx, val, lc, uc, c, l, u)
     s = capi.Settings(method=capi.CUOPT_METHOD_PDLP, log_to_console=False, infeasibility_detection=True,
-                      strict_infeasibility=strict, iteration_limit=CERT_CAP)
+                      strict_infeasibility=strict, iteration_limit=CERT_CAP, pdlp_solver_mode=mode)
     sol = capi.solve(p, s)
     assert sol.return_code == 0, sol.error_string
     assert sol.termination_status == PDLP_STATUS[name], sol.termination_reason
-    if strict:
+    if sol.termination_status in (2, 3):
+        ok, ratio = certifies(LP(name, off, idx, val, c, l, u, lc, uc), sol.primal(), sol.dual(),
+                              sol.termination_status, rule_of(mode))
+        assert ok, ratio
+    if strict and mode == po.STABLE2:
         o = po.Oracle(off, idx, val, c, l, u, lc, uc, tol=1e-4, detect_infeasibility=True, strict_infeasibility=True,
                       iteration_limit=CERT_CAP)
         o.run(-1)

@@ -222,11 +222,40 @@ def fixture(name):
         return from_rows([{0: 1}, {}], 2, [1, -1], [0, 0], [inf, inf], [1, -1], [3, 1])
     if name == "no_constraints":
         return arrays([0], [], [], [1.0, -1.0, 0.0, 2.0], [0, -5, -inf, -3], [inf, 5, inf, 4], [], [])
+    # certificates through presolve: PDLP decides these on the reduced problem
+    if name == "ray_singleton_lower":
+        # x0 >= 1 (a singleton G row) but x0 + x1 <= 0, x >= 0
+        return from_rows([{0: 1}, {0: 1, 1: 1}], 2, [1, 1], [0, 0], [inf, inf], [1, -inf], [inf, 0])
+    if name == "ray_singleton_negative_upper":
+        # -x0 >= 1 (x0 <= -1) but x0 - x1 >= 0, x1 >= 0
+        return from_rows([{0: -1}, {0: 1, 1: -1}], 2, [1, 1], [-inf, 0], [inf, inf], [1, 0], [inf, inf])
+    if name == "ray_singleton_ranged":
+        # 2 <= 2 x0 <= 6 (a ranged singleton row) but x0 + x1 <= 0, x >= 0
+        return from_rows([{0: 2}, {0: 1, 1: 1}], 2, [1, 1], [0, 0], [inf, inf], [2, -inf], [6, 0])
+    if name == "ray_fixed_column":
+        # x2 = 2 (fixed) turns x0 + x1 + x2 <= 1 into x0 + x1 <= -1, x >= 0
+        return from_rows([{0: 1, 1: 1, 2: 1}, {0: 1, 1: -1}], 3, [1, 1, 1], [0, 0, 2], [inf, inf, 2], [-inf, -4],
+                         [1, 4])
+    if name == "ray_fixed_makes_singleton":
+        # x2 = 1 (fixed) turns x0 + x2 >= 3 into the singleton x0 >= 2, but x0 + x1 <= 1, x >= 0
+        return from_rows([{0: 1, 2: 1}, {0: 1, 1: 1}], 3, [1, 1, 1], [0, 0, 1], [inf, inf, 1], [3, -inf], [inf, 1])
+    if name == "ray_unbounded_with_removed_columns":
+        # the unbounded_free_var certificate of test_bound_structures with a fixed column (x4 = 2) in its E row and a
+        # bounded empty column (x5, c5 > 0) next to it; both are removed, the reduced problem is that certificate
+        return from_rows([{0: 1, 1: 1, 3: -1, 4: 1}, {2: 1, 3: 1}], 6, [1, 0, 1, 0, 3, 1], [-inf, 0, -1, 0, 2, 0],
+                         [inf, inf, 1, inf, 2, 4], [3, -2], [3, 2])
     raise KeyError(name)
 
 
 OPTIMAL = ["bound_zoo", "bound_zoo_max_offset", "singleton_zoo_1", "singleton_zoo_2", "singleton_zoo_3", "afiro",
            "sudoku", "planted_large"]
+# (fixture, status, what presolve removes: fixed columns, singleton rows, empty columns)
+RAYS = [("ray_singleton_lower", "PrimalInfeasible", (0, 1, 0)),
+        ("ray_singleton_negative_upper", "PrimalInfeasible", (0, 1, 0)),
+        ("ray_singleton_ranged", "PrimalInfeasible", (0, 1, 0)),
+        ("ray_fixed_column", "PrimalInfeasible", (1, 0, 0)),
+        ("ray_fixed_makes_singleton", "PrimalInfeasible", (1, 1, 0)),
+        ("ray_unbounded_with_removed_columns", "DualInfeasible", (1, 0, 1))]
 VERDICTS = [("infeasible_empty_row", "PrimalInfeasible"), ("crossing_singletons", "PrimalInfeasible"),
             ("unbounded_empty_column", "DualInfeasible"), ("no_constraints", "Optimal")]
 
@@ -276,6 +305,16 @@ def test_verdicts_agree_with_highs(name, verdict):
     assert r["verdict"] == verdict
     res = highs_of(f)
     assert res.status == HIGHS_STATUS[verdict], res.message
+
+
+@pytest.mark.parametrize("name,verdict,removed", RAYS)
+def test_ray_fixtures_reduce_as_named_and_leave_the_verdict_to_pdlp(name, verdict, removed):
+    f, r = fixture(name), reference(name)
+    assert r["verdict"] is None and r["empty_rows"] == 0
+    assert (r["fixed_columns"], r["singleton_rows"], r["empty_columns"]) == removed
+    assert highs_of(f).status == HIGHS_STATUS[verdict]
+    red = highs(r["offsets"], r["indices"], r["values"], r["c"], r["l"], r["u"], r["lc"], r["uc"])
+    assert red.status == HIGHS_STATUS[verdict], red.message
 
 
 def test_nothing_to_remove_on_the_identity_fixtures():
@@ -449,6 +488,23 @@ def test_verdicts_with_full_size_vectors(name, verdict):
     if verdict == "Optimal":
         assert sol.stats().primal_objective == pytest.approx(highs_of(f).fun, rel=1e-9, abs=1e-12)
         assert np.all((x >= f["l"]) & (x <= f["u"]))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,verdict,removed", RAYS)
+def test_returned_ray_certifies_the_original_problem(name, verdict, removed):
+    """With presolve on, the certificate PDLP finds on the reduced problem comes back through postsolve and certifies the
+    ORIGINAL problem under the exact restatement of test_infeasibility_detection (Stable2: reduced-cost rule 0).  A dual
+    ray needs the duals of the singleton rows whose bounds it rests on."""
+    from test_infeasibility_detection import LP, certifies
+    f = fixture(name)
+    sol = capi.solve(problem_of(f), settings(tol=1e-4, infeasibility_detection=True, strict_infeasibility=True,
+                                             iteration_limit=100000, pdlp_solver_mode=po.STABLE2))
+    assert sol.return_code == 0 and sol.termination_status == VERDICT[verdict], (sol.termination_reason, sol.error_string)
+    assert sol.presolve_stats().ran == 1
+    lp = LP(name, f["offsets"], f["indices"], f["values"], min_form(f), f["l"], f["u"], f["lc"], f["uc"])
+    ok, ratio = certifies(lp, sol.primal(), sol.dual(), VERDICT[verdict], 0)
+    assert ok, (ratio, sol.primal().tolist(), sol.dual().tolist())
 
 
 @pytest.mark.gpu
