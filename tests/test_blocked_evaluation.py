@@ -10,16 +10,11 @@ import scipy.sparse as sp
 
 from conftest import problem_arrays
 from cuopt_b200 import capi, lpgen
+from exact import ELEMENTWISE, rel_err
 
 pytestmark = pytest.mark.gpu
 
-ELEMENTWISE = 1e-12
 STATS = ("primal_objective", "dual_objective", "gap", "l2_primal_residual", "l2_dual_residual")
-
-
-def rel_err(a, b):
-    a, b = np.asarray(a, float), np.asarray(b, float)
-    return float(np.max(np.abs(a - b)) / max(1.0, np.max(np.abs(b)))) if a.size else 0.0
 
 
 def problem(lp, **changes):

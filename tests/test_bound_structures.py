@@ -3,7 +3,7 @@
 The synthetic LPs of the other test files all have 0 <= x < +inf and rows of kind E, L or G, so the branches of the
 kernels that depend on the BOUND KIND ran only on afiro and a few MIP relaxations, and were checked there only through
 parity with the oracle or final objectives.  This file builds a seeded zoo of LPs that hold every kind in every role of
-a planted optimum (numpy, complementary slackness as planted() of test_spmv_structures.py):
+a planted optimum (numpy, complementary slackness as planted() of cases.py):
 
   variables  free; [l, +inf) with l < 0, l = 0, l > 0, at the bound or inside; (-inf, u] at the bound or inside;
              boxes at either bound or inside, straddling 0, entirely above 0, entirely below 0; one box 1e-6 |l| wide;
@@ -22,280 +22,40 @@ A maximisation is solved as the minimisation of -c (problem_helpers.cuh:127 of t
 scaling factor becomes -1), so the solver's y and reduced costs are those of min -c'x, and both reported objectives are
 -(that objective) + offset.
 
-Tolerances: as test_spmv_structures.py (componentwise row-sum bound 4 len 2^-53 sum|a_ij v_j| for every product).
+The cases are planted_bounds() and certificates() of cases.py.  Tolerances: those of exact.py (componentwise
+row-sum bound 4 len 2^-53 sum|a_ij v_j| for every product).
 """
-import functools
 import math
-from collections import namedtuple
 
 import numpy as np
 import pytest
 import scipy.sparse as sp
-from scipy.optimize import linprog
 
-from conftest import mps_path, problem_arrays
+from cases import (BOUND_ZOO as ZOO, CERT_STATUS, CERTIFICATES, HIGHS_STATUS, VAR_ROLES, bound_zoo as zoo,
+                   bounds_oracle as oracle_of, bounds_problem as problem_of, certificate_args, certificates, mps_arrays,
+                   settings_of)
 from cuopt_b200 import capi, lpgen
+from device_model import block_bytes, gather_block_bytes  # noqa: F401
+from device_model import session as dm_session
+from exact import (ACROSS_TRUST_REGION, OBJECTIVE, STEPWISE, TRAJECTORY, U53, LP, bound_value_product, certifies,
+                   close_counts, device_formulation, dual_step_reference, highs, reduced_costs_np, rel_err, row_sum_tolerance,
+                   row_sums_hp, rule_of, scaled_problem, scaled_transpose, transpose_product)
 from oracle import pdlp_oracle as po
-from test_spmv_structures import (ACROSS_TRUST_REGION, OBJECTIVE, STEPWISE, TRAJECTORY, U53, Case, column_blocks,
-                                  dual_step_reference, from_row_lengths, heavy_tail, rel_err, row_sum_tolerance,
-                                  row_sums_hp, scaled_transpose)
-from test_trust_region_reformulation import device_formulation
 
 inf = np.inf
 FAST1_TRAJECTORY = 1e-5
 BOUND_SLACK = 1e-12  # relative to max(1, |bound|)
 MODES = [po.STABLE1, po.STABLE2, po.METHODICAL1, po.FAST1]
-ENV = "CUOPT_B200_GATHER_BLOCK_BYTES"
 
-VAR_ROLES = ["free", "lower_neg_at", "lower_neg_in", "lower_zero_at", "lower_zero_in", "lower_pos_at", "lower_pos_in",
-             "upper_neg_at", "upper_pos_at", "upper_in",
-             "box_at_l", "box_at_u", "box_in", "box_above_at_l", "box_above_at_u", "box_above_in", "box_below_at_l",
-             "box_below_at_u", "box_below_in", "box_thin", "fixed_r_pos", "fixed_r_neg", "fixed_zero"]
-ROW_ROLES = ["E", "L_active", "L_inactive", "G_active", "G_inactive", "ranged_at_lc", "ranged_at_uc", "ranged_inside",
-             "free", "empty_ranged"]
-
-
-# ------------------------------------------------------------------------------------------------------- bound zoo
-def roles(count, names, rng):
-    """Every role at least once (at random positions), the rest drawn at random."""
-    assert count >= len(names)
-    r = np.concatenate([np.arange(len(names)), rng.integers(0, len(names), count - len(names))])
-    return np.array(names, dtype=object)[rng.permutation(r)]
-
-
-def planted_bounds(m, n, seed, maximize=False, offset=0.0, per_row=6, heavy_rows=0):
-    """An LP with every bound kind in every role of a known optimum (x*, y*, r* = c - A^T y*).
-    `heavy_rows` of the m rows (the last ones) get the Zipf row lengths of test_spmv_structures.heavy_tail.
-    Returns lpgen.LP with c of the problem to MINIMISE; `user_c` / `maximize` / `offset` describe the problem as posed
-    (max -c'x + offset when maximising), `optimal_objective` is its optimum."""
-    rng = np.random.default_rng(seed)
-    vr, rr = roles(n, VAR_ROLES, rng), roles(m, ROW_ROLES, rng)
-    lens = np.where(rr == "empty_ranged", 0, per_row)
-    base = from_row_lengths("", lens[:m - heavy_rows], n, seed + 1)
-    if heavy_rows:
-        h = heavy_tail("", heavy_rows, n, seed + 2)
-        off = np.concatenate([base.offsets, base.offsets[-1] + h.offsets[1:]]).astype(np.int32)
-        base = Case("", off, np.concatenate([base.indices, h.indices]), np.concatenate([base.values, h.values]), m, n)
-        rr[m - heavy_rows:][np.diff(h.offsets) == 0] = "empty_ranged"   # an empty heavy-tail row is an empty row
-        rr[m - heavy_rows:][(np.diff(h.offsets) > 0) & (rr[m - heavy_rows:] == "empty_ranged")] = "ranged_inside"
-    assert np.all((np.diff(base.offsets) == 0) == (rr == "empty_ranged"))
-
-    # variables: bounds, x*, r*
-    l, u, x, r = np.zeros(n), np.full(n, inf), np.zeros(n), np.zeros(n)
-    pos = lambda k=n: rng.uniform(0.5, 2.0, k)  # noqa: E731  strictly positive reduced costs / duals / slacks
-    for j, role in enumerate(vr):
-        a, b = sorted(rng.uniform(-10.0, 10.0, 2))
-        lo_, hi_ = -abs(a) - 0.5, abs(b) + 0.5                           # a box that straddles 0
-        above, below = (abs(a) + 0.5, abs(a) + abs(b) + 1.0), (-abs(a) - abs(b) - 1.0, -abs(a) - 0.5)
-        rp, mid = float(pos(1)[0]), float(rng.uniform(0.2, 0.8))
-        if role == "free":
-            l[j], u[j], x[j] = -inf, inf, rng.normal(0.0, 3.0)
-        elif role.startswith("lower"):
-            l[j] = {"neg": -abs(a) - 0.5, "zero": 0.0, "pos": abs(a) + 0.5}[role.split("_")[1]]
-            x[j], r[j] = (l[j], rp) if role.endswith("_at") else (l[j] + rng.uniform(0.5, 5.0), 0.0)
-        elif role.startswith("upper"):
-            l[j], u[j] = -inf, {"upper_neg_at": -abs(b) - 0.5, "upper_pos_at": abs(b) + 0.5}.get(role, b)
-            x[j], r[j] = (u[j], -rp) if role.endswith("_at") else (u[j] - rng.uniform(0.5, 5.0), 0.0)
-        elif role.startswith("box"):
-            l[j], u[j] = above if "above" in role else below if "below" in role else (lo_, hi_)
-            if role == "box_thin":
-                l[j] = abs(a) + 1.0
-                u[j] = l[j] * (1.0 + 1e-6)
-            if role.endswith("at_l") or role == "box_thin":
-                x[j], r[j] = l[j], rp
-            elif role.endswith("at_u"):
-                x[j], r[j] = u[j], -rp
-            else:
-                x[j] = l[j] + mid * (u[j] - l[j])
-        else:  # fixed
-            l[j] = u[j] = 0.0 if role == "fixed_zero" else a
-            x[j], r[j] = l[j], {"fixed_r_pos": rp, "fixed_r_neg": -rp}.get(role, rng.choice([-1.0, 1.0]) * rp)
-
-    # rows: bounds and y*
-    row = np.repeat(np.arange(m), np.diff(base.offsets))
-    ax = np.bincount(row, weights=base.values * x[base.indices], minlength=m)
-    y, s1, s2 = np.zeros(m), pos(m), pos(m)
-    lc, uc = ax.copy(), ax.copy()
-    for i, role in enumerate(rr):
-        if role == "E":
-            y[i] = rng.normal() + np.sign(rng.normal()) * 0.5
-        elif role == "L_active":
-            lc[i], y[i] = -inf, -s1[i]
-        elif role == "L_inactive":
-            lc[i], uc[i] = -inf, ax[i] + s2[i]
-        elif role == "G_active":
-            uc[i], y[i] = inf, s1[i]
-        elif role == "G_inactive":
-            lc[i], uc[i] = ax[i] - s2[i], inf
-        elif role == "ranged_at_lc":
-            uc[i], y[i] = ax[i] + s2[i], s1[i]
-        elif role == "ranged_at_uc":
-            lc[i], y[i] = ax[i] - s2[i], -s1[i]
-        elif role == "ranged_inside":
-            lc[i], uc[i] = ax[i] - s1[i], ax[i] + s2[i]
-        elif role == "free":
-            lc[i], uc[i] = -inf, inf
-        else:  # empty ranged row containing 0 (ax = 0)
-            lc[i], uc[i] = -s1[i], s2[i]
-    c = np.bincount(base.indices, weights=base.values * y[row], minlength=n) + r
-    lp = lpgen.LP(base.offsets, base.indices, base.values, c, l, u, lc, uc, None, x, y,
-                  name=f"planted_bounds({m}x{n},seed={seed},max={maximize},offset={offset})")
-    lp.r_star, lp.var_role, lp.row_role = r, vr, rr
-    lp.maximize, lp.offset = maximize, offset
-    lp.user_c = -c if maximize else c
-    lp.optimal_objective = float(lp.user_c @ x) + offset
-    return lp
-
-
-ZOO = ["tiny", "medium", "heavy", "medium_max", "medium_offset"]
-
-
-@functools.lru_cache(maxsize=None)
-def zoo(name):
-    if name == "tiny":
-        return planted_bounds(40, 30, 21)
-    if name == "heavy":
-        return planted_bounds(1600, 1200, 23, heavy_rows=600)
-    return planted_bounds(3000, 2500, 22, maximize=name == "medium_max",
-                          offset={"medium_offset": 123.25}.get(name, 0.0))
-
-
-def problem_of(lp):
-    return capi.Problem.create_ranged(lp.offsets, lp.indices, lp.values, lp.con_lb, lp.con_ub, lp.user_c, lp.var_lb,
-                                      lp.var_ub, maximize=lp.maximize, objective_offset=lp.offset)
-
-
-def oracle_of(lp, mode, tol=1e-9, **kw):
-    return po.Oracle(lp.offsets, lp.indices, lp.values, lp.user_c, lp.var_lb, lp.var_ub, lp.con_lb, lp.con_ub,
-                     maximize=lp.maximize, objective_offset=lp.offset, mode=mode, tol=tol, **kw)
-
-
-def case_of(lp):
-    return Case(lp.name, lp.offsets, lp.indices, lp.values, lp.m, lp.n)
-
-
-def transpose_of(lp, values=None):
-    A = sp.csr_matrix((lp.values if values is None else values, lp.indices, lp.offsets), shape=(lp.m, lp.n))
-    T = A.T.tocsr()
-    T.sort_indices()
-    return T.indptr, T.indices, T.data
-
-
-def highs(offsets, indices, values, c, l, u, lc, uc):
-    """linprog(method="highs") of min c'x, lc <= Ax <= uc, l <= x <= u (ranged rows as two inequalities)."""
-    A = sp.csr_matrix((values, indices, offsets), shape=(len(lc), len(c)))
-    eq = lc == uc
-    up, lo = np.isfinite(uc) & ~eq, np.isfinite(lc) & ~eq
-    A_ub = sp.vstack([A[up], -A[lo]]).tocsr()
-    b_ub = np.concatenate([uc[up], -lc[lo]])
-    return linprog(c, A_ub=A_ub if A_ub.shape[0] else None, b_ub=b_ub if A_ub.shape[0] else None,
-                   A_eq=A[eq] if eq.any() else None, b_eq=lc[eq] if eq.any() else None,
-                   bounds=np.column_stack([l, u]), method="highs")
-
-
-# ------------------------------------------------------------------------------------------------------ certificates
-Cert = namedtuple("Cert", "name offsets indices values c l u lc uc status")  # 1 optimal, 2 infeasible, 3 unbounded
-HIGHS_STATUS = {1: 0, 2: 2, 3: 3}  # linprog: 0 optimal, 2 infeasible, 3 unbounded
-
-
-def cert(name, rows, c, l, u, lc, uc, status):
-    """rows: list of {column: value}."""
-    off = np.concatenate([[0], np.cumsum([len(r) for r in rows])]).astype(np.int32)
-    idx = np.array([j for r in rows for j in sorted(r)], np.int32)
-    val = np.array([r[j] for r in rows for j in sorted(r)], float)
-    return Cert(name, off, idx, val, *(np.asarray(v, float) for v in (c, l, u, lc, uc)), status)
-
-
-@functools.lru_cache(maxsize=None)
-def certificates():
-    """Small LPs whose infeasibility / unboundedness rests on ONE bound kind (without it they are feasible / bounded).
-    A feasible ranged row and a boxed variable ride along in each, so the verdict passes other kinds too."""
-    return [
-        # x0 fixed at 1, but x0 + x1 <= 0 with x1 >= 0
-        cert("infeasible_fixed_var", [{0: 1, 1: 1}, {1: 1, 2: 1}], [1, 1, 1], [1, 0, -1], [1, inf, 1],
-             [-inf, -2], [0, 2], 2),
-        # x0 <= -1 (upper-only), but x0 - x1 >= 0 with x1 >= 0
-        cert("infeasible_upper_only_var", [{0: 1, 1: -1}, {1: 1, 2: 1}], [1, 1, 1], [-inf, 0, -1], [-1, inf, 1],
-             [0, -2], [inf, 2], 2),
-        # 1 <= x0 + x1 <= 2 (ranged), but x0 + x1 >= 3
-        cert("infeasible_ranged_row", [{0: 1, 1: 1}, {0: 1, 1: 1}, {1: 1, 2: 1}], [1, 1, 1], [0, 0, -1], [inf, inf, 1],
-             [1, 3, -2], [2, inf, 2], 2),
-        # x0 + x1 = -1 with x >= 0
-        cert("infeasible_equality_row", [{0: 1, 1: 1}, {1: 1, 2: 1}], [1, 1, 1], [0, 0, -1], [inf, inf, 1],
-             [-1, -2], [-1, 2], 2),
-        # min x0 with x0 free and x0 + x1 - x3 = 1, x1, x3 >= 0
-        cert("unbounded_free_var", [{0: 1, 1: 1, 3: -1}, {2: 1, 3: 1}], [1, 0, 1, 0], [-inf, 0, -1, 0],
-             [inf, inf, 1, inf], [1, -2], [1, 2], 3),
-        # min -x1 with x0 + x1 = 1 and x0 <= 2 (upper-only): x1 grows as x0 falls
-        cert("unbounded_upper_only_var_negative_cost", [{0: 1, 1: 1}, {1: 1, 2: 1}], [0, -1, 1], [-inf, 0, -1],
-             [2, inf, 1], [1, -2], [1, inf], 3),
-        # min x0 + x2 with -inf < x0 <= 3 (lower bound -inf) and x0 + x1 = -4, x1 >= -2 (negative lower bound)
-        cert("unbounded_minus_inf_lower_bound", [{0: 1, 1: 1}, {2: 1, 3: 1}], [1, 0, 1, 0], [-inf, -2, -1, 0],
-             [3, inf, 1, inf], [-4, -2], [-4, 2], 3),
-        # the control: min -x0 + x1 / 1000 with x0 + x1 >= 100 and 0 <= x0 <= 5 is bounded only by the upper bound
-        # of x0; while the iterate is short of the G row (primal infeasible, homogeneous residual 0) the ray test
-        # runs, and it is the finite upper bound of x0 that must keep it from reporting Unbounded
-        cert("optimal_because_of_upper_bound", [{0: 1, 1: 1}], [-1, 1e-3], [0, 0], [5, inf], [100], [inf], 1),
-    ]
-
-
-MPS_CERTIFICATES = [("good-mps-free-var", 3), ("good-mps-lower-bound-inf-var", 3), ("good-mps-fixed-var", 2),
-                    ("good-mps-fixed-ranges", 2), ("good-mps-free-ranges", 2)]
 MPS_OPTIMA = [("lp_model_with_var_bounds", -2.0), ("good-mps-some-var-bounds", -0.2), ("good-mps-rhs-cost", -5.0)]
-
-
-def mps_arrays(name):
-    a = problem_arrays(capi.Problem.read(mps_path(f"linear_programming/{name}.mps")))
-    assert not a["maximize"]
-    return a
-
-
-def certificate_args(name):
-    if name.startswith("good-mps"):
-        a = mps_arrays(name)
-        return tuple(a[k] for k in ("offsets", "indices", "values", "c", "var_lb", "var_ub", "con_lb", "con_ub"))
-    k = next(k for k in certificates() if k.name == name)
-    return k.offsets, k.indices, k.values, k.c, k.l, k.u, k.lc, k.uc
-
-
-CERTIFICATES = [k.name for k in certificates()] + [n for n, _ in MPS_CERTIFICATES]
-CERT_STATUS = {**{k.name: k.status for k in certificates()}, **dict(MPS_CERTIFICATES)}
 # PDLP tests for a ray only while the iterate is primal INFEASIBLE (termination_strategy.cu:141-227 of the reference:
 # Optimal / PrimalFeasible are decided first).  On these two fixtures the diverging iterate stays primal feasible (one
 # L row, a free variable), so PDLP (the reference, the oracle and this build alike) ends with NumericalError (6) when
-# the iterate overflows, not with HiGHS's Unbounded; the certificates above put an equality row in the way of the ray.
+# the iterate overflows, not with HiGHS's Unbounded; the synthetic certificates put an equality row in the way of the ray.
 PDLP_STATUS = {**CERT_STATUS, "good-mps-free-var": 6, "good-mps-lower-bound-inf-var": 6}
 
 
 # ------------------------------------------------------------------------------------------------- numpy references
-def bound_value_product(v, lo, hi):
-    bound = np.where(v > 0.0, lo, np.where(v < 0.0, hi, 0.0))
-    with np.errstate(invalid="ignore"):
-        return np.where(np.isfinite(bound), v * bound, 0.0)
-
-
-def reduced_costs_np(lp, x, y, rule):
-    """(reduced costs under rule 0 / rule 1, g = c - A^T y, tolerance, exempt columns): exact products, fsum.
-    Where |g| lies within its tolerance of 0 the bound it presses on may flip, but both answers (0 or g) then lie
-    within twice that tolerance, which is what such a column is held to.  Exempt: under rule 1, |x - bound| and |x|
-    within a few roundings of each other but not equal (the comparison itself may flip)."""
-    aty, mag, lens = row_sums_hp(*transpose_of(lp), y)
-    g = lp.c - aty
-    tol = row_sum_tolerance(mag, lens) + 4 * U53 * (np.abs(lp.c) + np.abs(aty))
-    bound = np.where(g > 0.0, lp.var_lb, lp.var_ub)
-    with np.errstate(invalid="ignore"):
-        dist = np.abs(x - bound)
-        keep = dist <= np.abs(x) if rule else np.isfinite(bound)
-        diff = np.abs(dist - np.abs(x))  # 0 for a zero bound: the comparison is then exact
-        near = rule & np.isfinite(bound) & (diff > 0.0) & (diff < 4 * U53 * (np.abs(x) + np.abs(bound)))
-    rc = np.where((g != 0.0) & keep, g, 0.0)
-    return rc, g, np.where(np.abs(g) <= tol, 2.0 * tol, tol), near
-
-
-def rule_of(mode):
-    return po.preset(mode).handle_some_primal_gradients_on_finite_bounds_as_residuals
-
-
 def evaluation_np(lp, x, y, rc):
     """Primal / dual objectives of the posed problem, l2 residuals, gap, and the linf per-constraint criteria, from
     fsum over exact products, with `rc` the reduced costs the evaluation used; plus absolute tolerances."""
@@ -303,7 +63,7 @@ def evaluation_np(lp, x, y, rc):
     axtol = row_sum_tolerance(mag, lens)
     with np.errstate(invalid="ignore"):
         viol = np.where(ax < lp.con_lb, lp.con_lb - ax, np.where(ax > lp.con_ub, ax - lp.con_ub, 0.0))
-    aty, magt, lenst = row_sums_hp(*transpose_of(lp), y)
+    aty, magt, lenst = transpose_product(lp.offsets, lp.indices, lp.values, lp.n, y)
     g = lp.c - aty
     sgn = -1.0 if lp.maximize else 1.0
     prods = lp.c * x
@@ -331,12 +91,6 @@ def assert_evaluation(lp, x, y, rc, st):
         tol = tol + 1e-12 * abs(ref[v])  # the device sums in its own order: a relative rounding allowance
         assert abs(got - ref[v]) <= tol, (v, got, ref[v], tol)
     return ref
-
-
-def scaled_problem(lp, g):
-    """scipy CSR of the scaled A and the scaled vectors of a session."""
-    As = sp.csr_matrix((g.vector("scaled_values"), lp.indices, lp.offsets), shape=(lp.m, lp.n))
-    return As, g.vector("scaled_c"), g.vector("scaled_l"), g.vector("scaled_u"), g.vector("scaled_lc"), g.vector("scaled_uc")
 
 
 # ------------------------------------------------------------------------------------------------------- CPU tests
@@ -452,7 +206,7 @@ def test_oracle_meets_every_criterion(name, mode):
     ls, us = o.vector("scaled_l"), o.vector("scaled_u")
     x = np.clip(rng.normal(0.0, 3.0, lp.n), ls, us)
     y = rng.normal(0.0, 1.0, lp.m)
-    case = case_of(lp)
+    case = lp
     scaled = o.vector("scaled_values")
     T = scaled_transpose(case, scaled, o.vector("scaled_values_t"))
     aty, mag, lens = row_sums_hp(*T, y)
@@ -526,34 +280,8 @@ CERT_CAP = 100000
 
 
 # ------------------------------------------------------------------------------------------------------- GPU tests
-@pytest.fixture
-def gather_block_bytes(monkeypatch):
-    """Force gather blocking (None: leave it to the solver, which does not block at these sizes)."""
-    def force(nbytes):
-        if nbytes is None:
-            monkeypatch.delenv(ENV, raising=False)
-        else:
-            monkeypatch.setenv(ENV, str(int(nbytes)))
-    yield force
-    monkeypatch.delenv(ENV, raising=False)
-
-
-def block_bytes(lp, blocks):
-    return None if blocks is None else max(1, int(8 * min(lp.m, lp.n) / 2.5))
-
-
-def settings_of(mode, tol=1e-9, **kw):
-    s = capi.Settings(method=capi.CUOPT_METHOD_PDLP, log_to_console=False, pdlp_solver_mode=mode, **kw)
-    s.set("optimality_tolerance", tol)
-    return s
-
-
 def session(lp, mode, blocks, force):
-    nbytes = block_bytes(lp, blocks)
-    force(nbytes)
-    g = capi.Solver(problem_of(lp), settings_of(mode))
-    g.initialise()
-    assert g.scalar("eval_blocks") == column_blocks(lp.n, lp.nnz, nbytes)[0]
+    g = dm_session(lp, problem_of(lp), settings_of(mode, 1e-9), blocks, force)
     if blocks is not None:
         assert g.scalar("eval_blocks") >= 3 and g.scalar("eval_blocks_t") >= 3
     return g
@@ -608,7 +336,7 @@ def test_primal_and_dual_steps_respect_every_bound_kind(name, blocks, mode, gath
     """K1 and K2 of every step accepted at its first attempt, element by element, and the exact invariants."""
     lp = zoo(name)
     g = session(lp, mode, blocks, gather_block_bytes)
-    case = case_of(lp)
+    case = lp
     scaled = g.vector("scaled_values")
     T = scaled_transpose(case, scaled, g.vector("scaled_values_t"))
     c, l, u, lc, uc = (g.vector(v) for v in ("scaled_c", "scaled_l", "scaled_u", "scaled_lc", "scaled_uc"))
@@ -745,7 +473,7 @@ def test_trust_region_kernels_at_chosen_points(name):
     """k_tr_prepare / sort / k_tr_weights / k_tr_bisect / k_tr_bounds through the read-only session hook against the
     numpy transcription of the device formulation, at radii from 0 to 1e6."""
     lp = tr_session_lp(name)
-    g = capi.Solver(problem_of(lp), settings_of(po.METHODICAL1))
+    g = capi.Solver(problem_of(lp), settings_of(po.METHODICAL1, 1e-9))
     g.initialise()
     g.advance(5)
     prob = scaled_problem(lp, g)
@@ -809,9 +537,7 @@ VERDICT_CASES = [(n, m, strict) for n in CERTIFICATES for m in MODES for strict 
 @pytest.mark.parametrize("name,mode,strict", VERDICT_CASES)
 def test_certificate_verdict(name, mode, strict):
     """The verdict under every preset, and the returned vectors re-evaluated on the LP by the exact restatement of
-    test_infeasibility_detection with the preset's reduced-cost rule: they meet the criterion the solver reported."""
-    from test_infeasibility import close_counts
-    from test_infeasibility_detection import LP, certifies
+    exact.py with the preset's reduced-cost rule: they meet the criterion the solver reported."""
     off, idx, val, c, l, u, lc, uc = certificate_args(name)
     p = capi.Problem.create_ranged(off, idx, val, lc, uc, c, l, u)
     s = capi.Settings(method=capi.CUOPT_METHOD_PDLP, log_to_console=False, infeasibility_detection=True,

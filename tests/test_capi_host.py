@@ -8,15 +8,11 @@ import re
 import numpy as np
 import pytest
 
+from cases import RANGED_LP
 from conftest import ROOT
 from cuopt_b200 import capi
 
 INF = float("inf")
-# c_api_test.c:761-790 (test_ranged_problem)
-RANGED_LP = dict(offsets=np.array([0, 2, 4, 6], np.int32), indices=np.array([0, 1, 0, 1, 0, 1], np.int32),
-                 values=np.array([2.0, 3.0, 3.0, 1.0, 1.0, 2.0]), c=np.array([5.0, 8.0]),
-                 con_lb=np.array([-INF, -INF, 2.0]), con_ub=np.array([12.0, 6.0, 8.0]),
-                 var_lb=np.array([0.0, 0.0]), var_ub=np.array([10.0, 10.0]))
 
 
 def test_library_loads_and_exports_every_declared_symbol():

@@ -1,9 +1,9 @@
 """Compact column blocks (CUOPT_B200_COMPACT_BLOCKS, spmv_bicsr.cuh): three-byte block-local column indices and the
 non-empty-row mask in place of the row-slot table.
 
-CPU: a numpy model of the encoding — local indices, the flags of the high bytes, pad slots, masks and the ordinals
-under which the row sums pass through shared memory — round-trips to the plain BICSR arrays of every column block of
-the structure zoo of test_spmv_structures.py, and the host rule that chooses the form is checked at the 2^21-column
+CPU: the numpy model of the encoding in device_model.py — local indices, the flags of the high bytes, pad slots, masks
+and the ordinals under which the row sums pass through shared memory — round-trips to the plain BICSR arrays of every
+column block of the structure zoo of cases.py, and the host rule that chooses the form is checked at the 2^21-column
 edge of the three-byte indices.
 
 GPU: the compact form changes where bytes come from, not what is added, so every product of the solver must be
@@ -13,126 +13,13 @@ of 3 and 16 column blocks.
 """
 import numpy as np
 import pytest
-import scipy.sparse as sp
 
+from cases import ZOO, Case, as_transpose, planted, problem_of, settings_of, zoo
 from cuopt_b200 import capi
-from test_spmv_structures import (CH, SLOTS, ZOO, Case, block_bytes, column_blocks, cut_blocks, planted, problem_of,
-                                  settings_of, zoo)
+from device_model import (CH, GATHER, IDX3, IDX3_MAX_WIDTH, MASK, SLOTS, block_bytes, column_blocks, cut, decode_compact,
+                          encode_compact, encode_plain, host_form, ordinal_of_row, ordinals_of_ends, split_columns)
 
 SWITCH = "CUOPT_B200_COMPACT_BLOCKS"
-GATHER = "CUOPT_B200_GATHER_BLOCK_BYTES"
-IDX3, MASK = 1, 2
-IDX3_MAX_WIDTH = 1 << 21
-PAD = 0x7FFFFFFF
-EMPTY = 0xFFFF
-HI_PAD, HI_END = 0x40, 0x80
-
-
-# ------------------------------------------------------------------------------------------------------ numpy model
-def split_columns(case, width, b):
-    """CSR (offsets, global column indices) of column block b: the entries of every row with a column in
-    [b width, (b + 1) width), in row order."""
-    off = np.asarray(case.offsets, np.int64)
-    idx = np.asarray(case.indices, np.int64)
-    keep = (idx >= b * width) & (idx < (b + 1) * width)
-    row = np.repeat(np.arange(case.m), np.diff(off))
-    counts = np.bincount(row[keep], minlength=case.m)
-    return np.concatenate([[0], np.cumsum(counts)]).astype(np.int64), idx[keep]
-
-
-def slot(q):
-    return (q % CH) * 32 + q // CH
-
-
-def encode_plain(off, idx, blk):
-    """Slots (bit 31: row end, PAD unused) and row-slot table of one interleaved block (r0, r1)."""
-    r0, r1 = blk
-    lo, cnt = off[r0], off[r1] - off[r0]
-    slots = np.full(SLOTS, PAD, np.int64)
-    for q in range(cnt):
-        slots[slot(q)] = idx[lo + q]
-    row_slot = np.full(r1 - r0, EMPTY, np.int64)
-    for r in range(r0, r1):
-        if off[r + 1] > off[r]:
-            s = slot(off[r + 1] - 1 - lo)
-            slots[s] |= 1 << 31
-            row_slot[r - r0] = s
-    return slots, row_slot
-
-
-def encode_compact(off, idx, blk, col0):
-    """lo16 (lane-major: entry q at position q), hi8 (lane l: one word, byte k = entry 8 l + k) and the 8 mask words."""
-    r0, r1 = blk
-    lo, cnt = off[r0], off[r1] - off[r0]
-    ends = np.zeros(SLOTS, bool)
-    mask = np.zeros(8, np.uint64)
-    for r in range(r0, r1):
-        if off[r + 1] > off[r]:
-            ends[off[r + 1] - 1 - lo] = True
-            mask[(r - r0) // 32] |= np.uint64(1 << ((r - r0) % 32))
-    lo16 = np.zeros(SLOTS, np.uint16)
-    hi8 = np.zeros(32, np.uint64)
-    for q in range(SLOTS):
-        if q < cnt:
-            c = int(idx[lo + q]) - col0
-            assert 0 <= c < IDX3_MAX_WIDTH, "a three-byte index holds 21 bits"
-            lo16[q] = c & 0xFFFF
-            hb = (c >> 16) | (HI_END if ends[q] else 0)
-        else:
-            hb = HI_PAD
-        hi8[q // CH] |= np.uint64(hb << (8 * (q % CH)))
-    return lo16, hi8, mask.astype(np.uint32)
-
-
-def decode_compact(lo16, hi8, mask, col0, n_rows):
-    """The plain slots and row-slot table back from the compact arrays (what the kernels read, in the kernels' terms)."""
-    slots = np.full(SLOTS, PAD, np.int64)
-    for l in range(32):
-        for k in range(CH):
-            q = CH * l + k
-            hb = (int(hi8[l]) >> (8 * k)) & 0xFF
-            if hb & HI_PAD:
-                continue
-            col = (((hb & 0x1F) << 16) | int(lo16[q])) + col0
-            slots[k * 32 + l] = col | ((1 << 31) if hb & HI_END else 0)
-    # the mask says which rows are non-empty; their last entries are the row ends in entry order
-    end_entries = [q for q in range(SLOTS) if (int(hi8[q // CH]) >> (8 * (q % CH) + 7)) & 1]
-    row_slot = np.full(n_rows, EMPTY, np.int64)
-    for i in range(n_rows):
-        if (int(mask[i // 32]) >> (i % 32)) & 1:
-            row_slot[i] = slot(end_entries[ordinal_of_row(mask, i)])
-    return slots, row_slot
-
-
-def ordinal_of_row(mask, i):
-    """Epilogue side: popcount of the mask below row i (bicsr_mask_cursor_t)."""
-    below = sum(bin(int(w)).count("1") for w in mask[: i // 32])
-    return below + bin(int(mask[i // 32]) & ((1 << (i % 32)) - 1)).count("1")
-
-
-def ordinals_of_ends(hi8):
-    """Row-sum side: the ordinal of every row end from the per-lane end bits, as the ballots form it
-    (bicsr_block_row_sums<true>: prefix popcount over the 4 bits of the per-lane counts, then inside the lane)."""
-    ends = [sum(((int(hi8[l]) >> (8 * k + 7)) & 1) << k for k in range(CH)) for l in range(32)]
-    cnt = [bin(e).count("1") for e in ends]
-    out = {}
-    for l in range(32):
-        ballots = [sum(((cnt[j] >> b) & 1) << j for j in range(32)) for b in range(4)]
-        before = sum(bin(ballots[b] & ((1 << l) - 1)).count("1") << b for b in range(4))
-        for k in range(CH):
-            if (ends[l] >> k) & 1:
-                out[CH * l + k] = before + bin(ends[l] & ((1 << k) - 1)).count("1")
-    return out
-
-
-def host_form(compact_blocks, width, sharded=False, forced_width=False):
-    """build_gather_blocks: the form of the column blocks of a single-GPU product."""
-    if sharded or forced_width:
-        return 0
-    fmt = compact_blocks & (IDX3 | MASK)
-    if width > IDX3_MAX_WIDTH:
-        fmt &= ~IDX3
-    return fmt
 
 
 def column_block_cases():
@@ -141,23 +28,18 @@ def column_block_cases():
         case = zoo()[name]
         sides = [("A", case)]
         if case.m != case.n or name in ("long_rows", "empty_rows_and_columns"):
-            T = case._replace(m=case.n, n=case.m)
-            At = sp.csr_matrix((case.values, case.indices, case.offsets), shape=(case.m, case.n)).T.tocsr()
-            At.sort_indices()
-            sides.append(("AT", T._replace(offsets=At.indptr, indices=At.indices, values=At.data)))
+            sides.append(("AT", as_transpose(case)))
         for side, M in sides:
             for blocks in (3, 16):
-                B, width = column_blocks(M.n, len(M.values), block_bytes(case, blocks))
-                for b in range(B):
-                    off, idx = split_columns(M, width, b) if B > 1 else (np.asarray(M.offsets, np.int64),
-                                                                         np.asarray(M.indices, np.int64))
-                    yield name, side, blocks, b, off, idx, b * width if B > 1 else 0
+                width = column_blocks(M.n, len(M.values), block_bytes(case, blocks))[1]
+                for b, (off, idx) in enumerate(split_columns(M, width)):
+                    yield name, side, blocks, b, off, idx, b * width
 
 
 def test_compact_encoding_round_trips_on_the_zoo():
     seen = dict(empty_block=0, empty_rows=0, lane_spans=0, pads=0, blocks=0)
     for name, side, blocks, b, off, idx, col0 in column_block_cases():
-        std, _ = cut_blocks(off)
+        std, _ = cut(off)
         if len(idx) == 0:
             seen["empty_block"] += 1
         for blk in std:
@@ -192,7 +74,7 @@ def test_three_byte_indices_at_the_width_edge():
         cols[0][0], cols[-1][-1] = 0, width - 1
         idx = np.concatenate(cols) + b * width
         off = np.concatenate([[0], np.cumsum(lens)])
-        for blk in cut_blocks(off)[0]:
+        for blk in cut(off)[0]:
             lo16, hi8, mask = encode_compact(off, idx, blk, b * width)
             slots, row_slot = decode_compact(lo16, hi8, mask, b * width, blk[1] - blk[0])
             plain = encode_plain(off, idx, blk)

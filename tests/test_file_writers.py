@@ -8,6 +8,7 @@ import os
 import numpy as np
 import pytest
 
+from cases import RANGED_LP
 from conftest import load_golden, mps_path, problem_arrays
 from cuopt_b200 import capi, lpgen
 
@@ -96,7 +97,7 @@ def test_reference_parser_reads_what_we_write(tmp_path):
 def test_ranged_rows_are_written_like_the_reference_writes_them(tmp_path):
     # write_mps.cu:60-70, 109-140: a row with two finite, different bounds becomes 'L' with RHS = lower bound and
     # RANGES = upper - lower (flagged in file_writers.cpp: not the MPS convention for 'L' rows, kept for output parity)
-    from test_capi_host import RANGED_LP as d
+    d = RANGED_LP
     p = capi.Problem.create_ranged(d["offsets"], d["indices"], d["values"], d["con_lb"], d["con_ub"], d["c"],
                                    d["var_lb"], d["var_ub"], maximize=True)
     out = str(tmp_path / "ranged.mps")

@@ -15,21 +15,15 @@ import os
 import numpy as np
 import pytest
 
+from cases import host_threads, problem_of as lp_problem
 from cuopt_b200 import capi, lpgen
+from exact import rel_err
 from oracle import pdlp_oracle as po
-from test_gpu_parity import lp_problem, rel_err
 
 pytestmark = [pytest.mark.gpu, pytest.mark.slow]
 
 # tolerance at which PDLP's relative criteria imply 1e-6 on the objectives of the planted LPs (measured)
 TIGHT = 1e-7
-
-
-def host_threads():
-    try:
-        return max(1, min(32, len(os.sched_getaffinity(0))))
-    except Exception:  # noqa: BLE001
-        return 8
 
 
 def test_headline_lp_steps_match_the_oracle_elementwise():

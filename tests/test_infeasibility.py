@@ -3,24 +3,12 @@ termination_strategy/infeasibility_information.cu and the verdicts of the refere
 import numpy as np
 import pytest
 
+from cases import c_api_infeasible_lp, unbounded_lp
 from cuopt_b200 import capi
+from exact import close_counts
 from oracle import pdlp_oracle as po
-from test_oracle_pins import c_api_infeasible_lp
 
 pytestmark = pytest.mark.gpu
-
-
-def unbounded_lp():
-    inf = np.inf
-    return (np.array([0, 2], np.int32), np.array([0, 1], np.int32), np.array([1.0, -1.0]), np.array([-1.0, 0.0]),
-            np.zeros(2), np.full(2, inf), np.zeros(1), np.zeros(1))
-
-
-def close_counts(gpu_steps, oracle_steps):
-    """The certificate is reached on a DIVERGING iterate sequence, where rounding differences between the two
-    implementations grow instead of being damped: same verdict, the
-    iteration at which the 1e-8 threshold is crossed within a few major iterations / 50 %."""
-    return abs(gpu_steps - oracle_steps) <= max(160, 0.5 * oracle_steps)
 
 
 def solve(lp, **params):

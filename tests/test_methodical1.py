@@ -6,10 +6,11 @@
 import numpy as np
 import pytest
 
-from conftest import mps_path
+from cases import lp_relaxation, make_pair
+from conftest import mps_path, problem_arrays
 from cuopt_b200 import capi
+from exact import rel_err
 from oracle import pdlp_oracle as po
-from test_gpu_parity import make_pair, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -52,8 +53,6 @@ def test_iterates_across_trust_region_restarts_match_the_oracle():
 
 @pytest.mark.parametrize("rel", ["mip/sudoku.mps", "mip/sample.mps", "mip/bb_optimality.mps"])
 def test_objective_against_the_oracle(rel):
-    from test_gpu_parity import lp_relaxation
-    from conftest import problem_arrays
     p = lp_relaxation(rel)
     a = problem_arrays(p)
     o = po.Oracle(a["offsets"], a["indices"], a["values"], a["c"], a["var_lb"], a["var_ub"], a["con_lb"], a["con_ub"],

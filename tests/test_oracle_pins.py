@@ -7,6 +7,7 @@ Sources of truth (all committed under tests/golden/, produced by scripts/gen_gol
 import numpy as np
 import pytest
 
+from cases import RANGED_LP, c_api_infeasible_lp, unbounded_lp
 from conftest import load_golden, mps_path, problem_arrays
 from cuopt_b200 import capi
 from oracle import pdlp_oracle as po
@@ -63,7 +64,6 @@ def test_maximisation_pins(pins, rel, key):
 def test_c_api_ranged_problem(pins):
     # c_api_test.c:761-874 / c_api_tests.cpp:89-96: maximize 5x + 8y ; 2x+3y <= 12 ; 3x+y <= 6 ; 2 <= x+2y <= 8 ;
     # 0 <= x,y <= 10  -> objective 32.0 +- 1e-3
-    from test_capi_host import RANGED_LP
     d = RANGED_LP
     o = po.Oracle(d["offsets"], d["indices"], d["values"], d["c"], d["var_lb"], d["var_ub"], d["con_lb"], d["con_ub"],
                   maximize=True, tol=1e-6)
@@ -159,19 +159,6 @@ def test_pds_shaped_lp_against_reference_dual_simplex():
 
 
 # ------------------------------------------------------------------ infeasibility detection (oracle only so far)
-def c_api_infeasible_lp():
-    """The LP of the reference's test_infeasible_problem (cpp/tests/linear_programming/c_api_tests/c_api_test.c:625-700)."""
-    inf = np.inf
-    off = np.array([0, 2, 4, 6, 7, 9, 10, 12, 15, 17], np.int32)
-    idx = np.array([0, 1, 0, 1, 0, 1, 3, 2, 3, 2, 0, 3, 0, 1, 2, 1, 2], np.int32)
-    val = np.array([-0.5, 1.0, 2.0, -1.0, 3.0, 1.0, 1.0, 3.0, -1.0, 1.0, 1.0, 1.0, 1.0, 2.0, 1.0, 1.0, 1.0])
-    rhs = np.array([0.5, 3.0, 6.0, 2.0, 2.0, 5.0, 10.0, 14.0, 1.0])
-    sense = "GGLLLGLLG"
-    lc = np.array([r if s in "GE" else -inf for r, s in zip(rhs, sense)])
-    uc = np.array([r if s in "LE" else inf for r, s in zip(rhs, sense)])
-    return off, idx, val, np.zeros(4), np.zeros(4), np.full(4, inf), lc, uc
-
-
 @pytest.mark.parametrize("strict", [False, True])
 def test_infeasibility_detection_on_the_reference_c_api_infeasible_lp(strict):
     off, idx, val, c, l, u, lc, uc = c_api_infeasible_lp()
@@ -185,12 +172,6 @@ def test_infeasibility_detection_on_the_reference_c_api_infeasible_lp(strict):
     o = po.Oracle(off, idx, val, c, l, u, lc, uc, tol=1e-4, iteration_limit=2000)
     assert o.run(-1)
     assert o.stats().termination_status == 4
-
-
-def unbounded_lp():
-    # min -x  s.t.  x - y = 0,  x, y >= 0: the ray (1, 1) improves forever
-    off, idx, val = np.array([0, 2], np.int32), np.array([0, 1], np.int32), np.array([1.0, -1.0])
-    return off, idx, val, np.array([-1.0, 0.0]), np.zeros(2), np.full(2, np.inf), np.zeros(1), np.zeros(1)
 
 
 def reference_verdict(name, off, idx, val, c, l, u, lc, uc):

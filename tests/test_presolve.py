@@ -15,9 +15,9 @@ import scipy.sparse as sp
 from conftest import mps_path, problem_arrays
 from cuopt_b200 import build as b
 from cuopt_b200 import capi, lpgen
+from cases import planted_bounds
+from exact import LP, STEPWISE, certifies, highs, rel_err, row_sum_tolerance
 from oracle import pdlp_oracle as po
-from test_bound_structures import highs, planted_bounds
-from test_spmv_structures import STEPWISE, rel_err, row_sum_tolerance
 
 inf = np.inf
 TOL = 1e-4              # absolute_primal_tolerance default: the infeasibility tests of presolve
@@ -240,7 +240,7 @@ def fixture(name):
         # x2 = 1 (fixed) turns x0 + x2 >= 3 into the singleton x0 >= 2, but x0 + x1 <= 1, x >= 0
         return from_rows([{0: 1, 2: 1}, {0: 1, 1: 1}], 3, [1, 1, 1], [0, 0, 1], [inf, inf, 1], [3, -inf], [inf, 1])
     if name == "ray_unbounded_with_removed_columns":
-        # the unbounded_free_var certificate of test_bound_structures with a fixed column (x4 = 2) in its E row and a
+        # the unbounded_free_var certificate of cases.py with a fixed column (x4 = 2) in its E row and a
         # bounded empty column (x5, c5 > 0) next to it; both are removed, the reduced problem is that certificate
         return from_rows([{0: 1, 1: 1, 3: -1, 4: 1}, {2: 1, 3: 1}], 6, [1, 0, 1, 0, 3, 1], [-inf, 0, -1, 0, 2, 0],
                          [inf, inf, 1, inf, 2, 4], [3, -2], [3, 2])
@@ -494,9 +494,8 @@ def test_verdicts_with_full_size_vectors(name, verdict):
 @pytest.mark.parametrize("name,verdict,removed", RAYS)
 def test_returned_ray_certifies_the_original_problem(name, verdict, removed):
     """With presolve on, the certificate PDLP finds on the reduced problem comes back through postsolve and certifies the
-    ORIGINAL problem under the exact restatement of test_infeasibility_detection (Stable2: reduced-cost rule 0).  A dual
-    ray needs the duals of the singleton rows whose bounds it rests on."""
-    from test_infeasibility_detection import LP, certifies
+    ORIGINAL problem under the exact restatement of exact.py (Stable2: reduced-cost rule 0).  A dual ray needs the duals
+    of the singleton rows whose bounds it rests on."""
     f = fixture(name)
     sol = capi.solve(problem_of(f), settings(tol=1e-4, infeasibility_detection=True, strict_infeasibility=True,
                                              iteration_limit=100000, pdlp_solver_mode=po.STABLE2))

@@ -20,7 +20,7 @@ def oracle_run(a, limit, flag):
 
 
 def relaxed(rel):
-    from test_gpu_parity import lp_relaxation
+    from cases import lp_relaxation
     return lp_relaxation(rel)
 
 

@@ -22,9 +22,9 @@ Cases (seeded, vectorised numpy, each with a planted optimum):
                  rows at every segment boundary: long rows at 65 535 / 65 536, a run of 1-entry rows across 131 072,
                  empty rows across 196 608; A^T has ~70 entries per row (32 lanes per row group, 3 rounds)
 
-References and tolerances are those of test_spmv_structures.py (componentwise row sums against the correctly rounded
-exact sum) and test_bound_structures.py; setup values that are one or two roundings of exact inputs are compared bit
-for bit.
+The cases are wide() of cases.py; the cut, grids and staging model are those of device_model.py.  References and
+tolerances are those of exact.py (componentwise row sums against the correctly rounded exact sum); setup values that
+are one or two roundings of exact inputs are compared bit for bit.
 """
 import functools
 import math
@@ -35,140 +35,33 @@ import sys
 import numpy as np
 import pytest
 
-from cuopt_b200 import capi, lpgen
+import device_model as dm
+from cases import (B1, B2, B3, EMPTY, RECYCLE, RUN, WIDE as CASES, cache_probe, host_threads, oracle_of, problem_of,
+                   recycle_solve, settings_of, solve_arrays, wide, zoo)
+from cuopt_b200 import capi
+from device_model import gather_block_bytes  # noqa: F401
+from device_model import (MAX_ROWS, RING, SEGMENT, SLOT, WARPS, cut, ew_grid, row_group_width, scaling_rounds,
+                          staged_arrays, staged_fills)
+from exact import (STEPWISE, TRAJECTORY, U53, assert_row_sums, check_evaluation, device_formulation, dot_tolerance,
+                   dual_step_reference, reduced_cost_reference, rel_err, row_sum_tolerance, row_sums_hp, scaled_problem,
+                   scaled_transpose, transpose)
 from oracle import pdlp_oracle as po
-from test_bound_structures import scaled_problem
-from test_headline_config import host_threads
-from test_spmv_structures import (MAX_ROWS, SLOTS, STEPWISE, TRAJECTORY, U53, Case, assert_row_sums,
-                                  block_bytes, check_evaluation, column_blocks, cut_blocks, dual_step_reference,
-                                  gather_block_bytes, oracle_of, planted, problem_of, reduced_cost_reference, rel_err,
-                                  row_sum_tolerance, row_sums_hp, scaled_transpose, settings_of, transpose_structure, zoo)
-from test_trust_region_reformulation import device_formulation
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SEGMENT = 1 << 16                  # SCHEDULE_SEGMENT of pdlp_solver.cu
-EW_THREADS, WARPS = 256, 8         # element-wise CTA size; warps (= blocks in flight) per SpMV CTA
-SLOT, RING = 32 << 20, 4           # staging ring of pdlp_solver.cu: slot bytes, slots; arrays below SLOT / 4 bypass it
-OCC, OCC2 = 4, 3                   # CTAs per SM the launch bounds aim at: SpMV kernels, fused K2 with two payload groups
 SMS = (132, 144)                   # the H100 SXM and margin above it
-CASES = ["tall", "short_rows", "segment_edges"]
+UNSEGMENTED = 1 << 40
 
 
-# ---------------------------------------------------------------------------------------------------------- cases
-def from_lengths(name, lens, n, seed):
-    """CSR with the given row lengths, distinct sorted columns uniform in [0, n), values N(0, 1) (vectorised)."""
-    rng = np.random.default_rng(seed)
-    lens = np.asarray(lens, np.int64)
-    row = np.repeat(np.arange(len(lens)), lens)
-    cols = rng.integers(0, n, int(lens.sum()))
-    for _ in range(64):
-        cols = cols[np.lexsort((cols, row))]
-        dup = np.zeros(len(cols), bool)
-        dup[1:] = (cols[1:] == cols[:-1]) & (row[1:] == row[:-1])
-        if not dup.any():
-            break
-        cols[dup] = rng.integers(0, n, int(dup.sum()))
-    assert not dup.any()
-    offsets = np.concatenate([[0], np.cumsum(lens)]).astype(np.int32)
-    return Case(name, offsets, cols.astype(np.int32), rng.standard_normal(len(cols)), len(lens), n)
-
-
-B1, B2, B3 = SEGMENT, 2 * SEGMENT, 3 * SEGMENT
-RUN = (B2 - 300, B2 + 300)         # 1-entry rows across the second boundary
-EMPTY = (B3 - 150, B3 + 50)        # empty rows across the third, ordinary rows after them
-
-
-@functools.lru_cache(maxsize=None)
-def wide(name):
-    """(Case, planted LP)."""
-    if name == "tall":
-        lp = lpgen.sparse_lp(600_000, 400_000, 8, seed=5)
-        return Case(name, lp.offsets, lp.indices, lp.values, lp.m, lp.n), lp
-    rng = np.random.default_rng({"short_rows": 31, "segment_edges": 32}[name])
-    if name == "short_rows":
-        case = from_lengths(name, rng.integers(1, 4, 1_100_000), 1_100_000, 33)
-    else:
-        m = 3 * SEGMENT + 77
-        lens = np.full(m, 6)
-        lens[rng.choice(m, 6200, replace=False)] = rng.integers(257, 301, 6200)
-        lens[B1 - 1], lens[B1] = 280, 290
-        lens[RUN[0]:RUN[1]] = 1
-        lens[EMPTY[0]:EMPTY[1]] = 0
-        case = from_lengths(name, lens, 40_000, 34)
-    return case, planted(case, 35)
-
-
-def transpose_offsets(case):
-    return np.concatenate([[0], np.cumsum(np.bincount(case.indices, minlength=case.n))])
-
-
-# ------------------------------------------------------------------------------------ numpy model of the launch geometry
-def cut_segmented(offsets, segment=SEGMENT):
-    """The BICSR cut of pdlp_solver.cu: cut_blocks() run on each `segment`-row segment, results joined in order.
-    -> (interleaved blocks [(first row, one past last row)], long rows)."""
-    off = np.asarray(offsets, np.int64)
-    rows = len(off) - 1
-    std, long_rows = [], []
-    for s0 in range(0, rows, segment):
-        s1, r = min(rows, s0 + segment), s0
-        while r < s1:
-            if off[r + 1] - off[r] > SLOTS:
-                long_rows.append(r)
-                r += 1
-                continue
-            r1 = min(int(np.searchsorted(off, off[r] + SLOTS, side="right")) - 1, r + MAX_ROWS, s1)
-            std.append((r, r1))
-            r = r1
-    return std, long_rows
-
-
-def ew_grid(count, sms):
-    return max(1, min(-(-count // EW_THREADS), 8 * sms))
-
-
-def spmv_grid(n_blk, sms, occ):
-    return max(1, min(-(-n_blk // WARPS), sms * occ))
-
-
-def row_group_width(rows, nnz):
-    avg = nnz / rows if rows else 0.0
-    return 4 if avg <= 4 else 8 if avg <= 8 else 16 if avg <= 16 else 32
-
-
-def scaling_rounds(rows, nnz, sms):
-    w = row_group_width(rows, nnz)
-    grid = max(1, min(-(-rows * w // 256), 16 * sms))
-    return -(-rows // (grid * (256 // w)))
-
-
-def staged_arrays(lp):
-    """Bytes of the host arrays a session uploads (A, bounds, costs)."""
-    return [4 * (lp.m + 1), 4 * lp.nnz, 8 * lp.nnz] + [8 * lp.n] * 3 + [8 * lp.m] * 2
-
-
-def staged_fills(lp):
-    return sum(-(-b // SLOT) for b in staged_arrays(lp) if b >= SLOT // 4)
-
-
+# ------------------------------------------------------------------------------------ the launch geometry of the cases
 @functools.lru_cache(maxsize=None)
 def structure_of(name):
     case, _ = wide(name)
-    a, at = cut_segmented(case.offsets), cut_segmented(transpose_offsets(case))
-    return dict(n_std_a=len(a[0]), n_blk_a=len(a[0]) + len(a[1]), n_long_a=len(a[1]),
-                n_std_at=len(at[0]), n_blk_at=len(at[0]) + len(at[1]), n_long_at=len(at[1]),
-                k2_npre=2 if a[0] and case.m > 40 * len(a[0]) else 1)
+    return dm.cut_counts(case.offsets, transpose(case.offsets, case.indices, case.n)[0])
 
 
-def geometry(name, sms, occ=OCC, occ2=OCC2):
+def geometry(name, sms, occ=dm.OCC, occ2=dm.OCC2):
     """What the solver launches for the case on `sms` SMs (unblocked)."""
-    case, lp = wide(name)
-    s = dict(structure_of(name))
-    s["grid_k2"] = spmv_grid(s["n_blk_a"], sms, occ2 if s["k2_npre"] == 2 else occ)
-    s["grid_k3"] = spmv_grid(s["n_blk_at"], sms, occ)
-    s["grid_n"], s["grid_m"] = ew_grid(case.n, sms), ew_grid(case.m, sms)
-    s["grid_k1"] = s["grid_n"]
-    s["staged_fills"] = staged_fills(lp)
-    return s
+    return dm.geometry(structure_of(name), wide(name)[1], sms, occ, occ2)
 
 
 def crossings(name, g, sms):
@@ -177,7 +70,7 @@ def crossings(name, g, sms):
     nnz = len(case.values)
     waves_a = g["n_std_a"] / (WARPS * g["grid_k2"])
     waves_at = g["n_std_at"] / (WARPS * g["grid_k3"])
-    ew = lambda count: -(-count // (ew_grid(count, sms) * EW_THREADS))  # noqa: E731  grid-stride rounds
+    ew = lambda count: -(-count // (ew_grid(count, sms) * dm.EW_THREADS))  # noqa: E731  grid-stride rounds
     out = {"partials > 256": ew_grid(max(case.m, case.n), sms) > 256, "segments": case.m > SEGMENT}
     big = [b for b in staged_arrays(lp) if b >= SLOT // 4]
     if name == "tall":
@@ -201,14 +94,14 @@ def crossings(name, g, sms):
 # ------------------------------------------------------------------------------------------------------- CPU tests
 def test_segmented_cut_equals_the_plain_cut_below_one_segment():
     for c in zoo().values():
-        assert cut_segmented(c.offsets) == cut_blocks(c.offsets), c.name
-    # and it is cut_blocks() per segment
+        assert cut(c.offsets) == cut(c.offsets, segment=UNSEGMENTED), c.name
+    # and it is the unsegmented cut per segment
     off = wide("segment_edges")[0].offsets
-    got = cut_segmented(off)
+    got = cut(off)
     want = ([], [])
     for s0 in range(0, len(off) - 1, SEGMENT):
         part = np.asarray(off[s0:min(len(off), s0 + SEGMENT + 1)], np.int64)
-        std, lng = cut_blocks(part - part[0])
+        std, lng = cut(part - part[0], segment=UNSEGMENTED)
         want[0].extend((a + s0, b + s0) for a, b in std)
         want[1].extend(r + s0 for r in lng)
     assert got == want
@@ -230,8 +123,8 @@ def test_census_every_case_crosses_what_it_is_named_for(name):
     if name == "segment_edges":
         off = np.asarray(case.offsets, np.int64)
         lens = np.diff(off)
-        std, lng = cut_segmented(off)
-        plain_std, _ = cut_segmented(off, segment=1 << 40)
+        std, lng = cut(off)
+        plain_std, _ = cut(off, segment=UNSEGMENTED)
         starts = {a for a, _ in std} | set(lng)
         assert {B1 - 1, B1} <= set(lng)                       # long rows on both sides of the first boundary
         assert (B1 - 1, B1) not in std and B1 in starts       # ... so a block ends exactly on it
@@ -277,7 +170,7 @@ def scaling_reference(case, mode):
     off = np.asarray(case.offsets, np.int64)
     row = np.repeat(np.arange(m), np.diff(off))
     col = np.asarray(case.indices, np.int64)
-    toff, tidx, pos = transpose_structure(case)
+    toff, tidx, pos = transpose(case.offsets, case.indices, case.n)
     a = np.asarray(case.values)
     lens, tlens = np.diff(off), np.diff(toff)
 
@@ -308,14 +201,9 @@ def scaling_reference(case, mode):
 
 # ------------------------------------------------------------------------------------------------------- GPU tests
 def session(name, blocks, force, mode=1, tol=1e-9, **kw):
-    """(case, LP, initialised GPU session) with the column blocking asked for, which is asserted."""
+    """(case, LP, initialised GPU session) with the column blocking asked for."""
     case, lp = wide(name)
-    nbytes = block_bytes(case, blocks)
-    force(nbytes)
-    g = capi.Solver(problem_of(lp), settings_of(mode, tol, **kw))
-    g.initialise()
-    assert g.scalar("eval_blocks") == column_blocks(case.n, lp.nnz, nbytes)[0]
-    assert g.scalar("eval_blocks_t") == column_blocks(case.m, lp.nnz, nbytes)[0]
+    g = dm.session(case, problem_of(lp), settings_of(mode, tol, **kw), blocks, force)
     if blocks is not None:
         assert g.scalar("eval_blocks") >= 3 and g.scalar("eval_blocks_t") >= 3
     return case, lp, g
@@ -358,7 +246,7 @@ def test_setup_bit_for_bit(name, mode, gather_block_bytes):
     row = np.repeat(np.arange(case.m), np.diff(case.offsets))
     col = np.asarray(case.indices, np.int64)
     assert np.array_equal(g.vector("scaled_values"), (case.values * dr[row]) * dc[col])
-    toff, tidx, pos = transpose_structure(case)
+    toff, tidx, pos = transpose(case.offsets, case.indices, case.n)
     assert np.array_equal(g.vector("scaled_values_t"), (case.values[pos] * dc[col[pos]]) * dr[tidx])
     with np.errstate(divide="ignore", invalid="ignore"):
         assert np.array_equal(g.vector("scaled_l"), np.where(dc == 0, 0.0, lp.var_lb / dc))
@@ -455,7 +343,7 @@ def test_evaluation_of_the_returned_iterate(name, checks):
     kw = dict(per_constraint_residual=True, infeasibility_detection=True) if checks else {}
     sol = capi.solve(problem_of(lp), settings_of(tol=1e-12, iteration_limit=40, **kw))
     assert sol.termination_reason == "IterationLimit"
-    check_evaluation(lp, sol, **(dict(per_constraint_residual=True, detect_infeasibility=True) if checks else {}))
+    check_evaluation(lp, sol, oracle_of(lp, **(dict(per_constraint_residual=True, detect_infeasibility=True) if checks else {})))
 
 
 @pytest.mark.gpu
@@ -504,12 +392,6 @@ def test_trust_region_kernels_at_a_million_components():
             assert abs(got[0] - want[0]) <= 1e-9 * scale and abs(got[1] - want[1]) <= 1e-9 * scale, (radius, got, want)
 
 
-def solve_arrays(sol):
-    st = sol.stats()
-    stats = {k: getattr(st, k) for k, _ in type(st)._fields_ if not (k == "solve_time" or k.endswith("_seconds"))}
-    return sol.primal(), sol.dual(), sol.reduced_costs(), stats
-
-
 @pytest.mark.gpu
 def test_two_solves_are_bit_identical_with_and_without_graphs(monkeypatch):
     """Repeated solves and the two launch paths give the same bits.  The cut's worker threads (as many as the host has
@@ -544,32 +426,11 @@ def test_full_solve_reaches_planted_optimum():
 
 
 # --------------------------------------------------------------------------------------------- recycled device memory
-RECYCLE = {"stable2_checks": dict(mode=po.STABLE2, per_constraint_residual=True, infeasibility_detection=True),
-           "methodical1": dict(mode=po.METHODICAL1)}
-
-
-def recycle_lp(seed):
-    return lpgen.sparse_lp(600_000, 400_000, 8, seed=seed)
-
-
-def cache_probe():
-    """A small session that stays open: it reads the process's block-cache counter without allocating anything."""
-    g = capi.Solver(problem_of(lpgen.sparse_lp(200, 150, 4, seed=1)), settings_of())
-    g.initialise()
-    return g
-
-
-def recycle_solve(config, seed):
-    kw = dict(RECYCLE[config])
-    return capi.solve(problem_of(recycle_lp(seed)), settings_of(tol=1e-12, iteration_limit=300, **kw))
-
-
 FRESH = """
 import sys
 sys.path[:0] = [{root!r}, {tests!r}]
 import numpy as np
-from test_wide_shapes import recycle_solve, solve_arrays
-from test_wide_shapes import cache_probe
+from cases import cache_probe, recycle_solve, solve_arrays
 x, y, rc, st = solve_arrays(recycle_solve({config!r}, {seed}))
 assert cache_probe().scalar("device_cache_hits") == 0
 np.savez({out!r}, x=x, y=y, rc=rc, **{{k: np.array(v) for k, v in st.items()}})
